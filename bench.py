@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- BASELINE.json's metric (Falcon-40B Q4_K decode tokens/s on B200) and, beside it, every BASELINE config.
+"""bench.py -- BASELINE.json's metric (Falcon-40B Q4_K decode tokens/s on one H100) and, beside it, every BASELINE config.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--config headline|1|2|3|4|5] [--no-extras]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--config headline|1|2|3|4|5] [--no-extras] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...      (N > 1)
 
 A "step" is one decode eval (one token, n_batch = 1) of a synthetic random-init Falcon model through the hot path; weights are
@@ -23,9 +23,13 @@ Top level = the headline config (or the one --config selects):
             REAL full-size model file (written to /dev/shm; identical layer tensors repeated, CPU time does not depend on values)
   prompt  : BASELINE config 3 (2048-token prompt, n_batch 512) with its own tensor roofline
   configs : cfg1 (Q4_0 4096x4096x1 mat-vec: reference ggml.c on the host cores + its GPU twin), cfg2 (Falcon-7B Q4_0 decode, 128 tokens),
-            cfg4 (Falcon-40B Q3_K decode, layer-split at N), cfg5 (Falcon-180B Q4_K decode at 8k context, KV pre-filled)
+            cfg4 (Falcon-40B Q3_K decode, layer-split at N), cfg5 (Falcon-180B Q4_K decode at 8k context, KV pre-filled; Falcon-40B on one GPU)
   pipeline_parity (N > 1): a small fixed model evaluated through the N-rank pipeline gives bit-identical logits / greedy tokens to
             the same model on one rank
+  --steps K: the timed steps -- decode tokens, whole 2048-token prompts (config 3) or passes over the 32 matrices (config 1)
+  --dump-outputs DIR: after the timed steps, what the timed path computed in its last step is written as DIR/<name>.npy (float32): the
+            logits of the last timed decode step (logits.npy), of the last prompt chunk (prompt_logits.npy) or the last timed mat-vec's
+            result (y.npy, config 1: the last of the 32 matrices).  Weights, token ids and positions are seeded, so equal arguments give equal inputs on every run.
 """
 import argparse
 import ctypes as C
@@ -56,6 +60,8 @@ DECODE_CONFIGS = {
     "4": ("falcon40b", Q3_K, 2048, 0, "falcon40b_q3_k_decode_tokens_per_s"),
     "5": ("falcon180b", Q4_K, 8192, 8000, "falcon180b_q4_k_decode_8k_ctx_tokens_per_s"),
 }
+# Falcon-180B Q4_K (100 GB of weights) does not fit one 80 GB H100: on one GPU the long-context config runs Falcon-40B at 8k context
+DECODE_CONFIG_1GPU = {"5": ("falcon40b", Q4_K, 8192, 8000, "falcon40b_q4_k_decode_8k_ctx_tokens_per_s")}
 WORKLOAD = {
     "headline": "Falcon-40B Q4_K decode, n_batch=1, synthetic random-init GGCC-shaped weights",
     "1": "Q4_0 4096x4096x1 mat-vec (examples/benchmark matmult shape), 32 rotating matrices",
@@ -64,14 +70,29 @@ WORKLOAD = {
     "4": "Falcon-40B Q3_K decode, n_batch=1, contiguous layer ranges per GPU",
     "5": "Falcon-180B Q4_K decode at 8k context (KV pre-filled to position 8000), contiguous layer ranges per GPU",
 }
+WORKLOAD_1GPU = {"5": "Falcon-40B Q4_K decode at 8k context (KV pre-filled to position 8000); Falcon-180B needs two or more 80 GB GPUs"}
+
+
+def decode_config(key, world):
+    """-> (model, weight type, n_ctx, first timed position, metric) of a decode config at `world` GPUs"""
+    return DECODE_CONFIG_1GPU[key] if world == 1 and key in DECODE_CONFIG_1GPU else DECODE_CONFIGS[key]
+
+
+def workload(key, world):
+    return WORKLOAD_1GPU[key] if world == 1 and key in WORKLOAD_1GPU else WORKLOAD[key]
+
+
+H100_HBM_GBS, H100_BF16_TFLOPS = 3350.0, 989.0        # NVIDIA H100 SXM data sheet (700 W card): HBM3 bandwidth, dense bf16
 
 
 def peaks():
+    """-> (HBM GB/s, dense bf16 TFLOP/s, source): a MEASURED_PEAKS.json beside this file wins, entry by entry, over the data sheet"""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return float(d["hbm_gbs"]), float(d.get("bf16_tflops_sustained", 1451.1)), "measured (MEASURED_PEAKS.json: hbm_gbs, bf16_tflops_sustained)"
-    return 6650.0, 1450.0, "fallback (B200_PROFILING.md: 6.65 TB/s copy, 1.45 PFLOP/s sustained bf16)"
+        return (float(d.get("hbm_gbs", H100_HBM_GBS)), float(d.get("bf16_tflops_sustained", H100_BF16_TFLOPS)),
+                "MEASURED_PEAKS.json (hbm_gbs, bf16_tflops_sustained; H100 SXM data sheet for a missing entry)")
+    return H100_HBM_GBS, H100_BF16_TFLOPS, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3, 989 TFLOP/s dense bf16; not measured)"
 
 
 def weight_elems(hp):
@@ -113,7 +134,7 @@ def stage_ranges(hp, world):
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons sampled during the timed region (B200_PROFILING.md recipe)"""
+    """nvidia-smi clocks + throttle reasons sampled during the timed region"""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -324,6 +345,11 @@ def reference_cpu_matvec(K=4096, M=4096, n_mats=32, iters=8):
 
 
 # ------------------------------------------------------------------------------------------------ GPU legs
+def dump(dump_dir, name, a):
+    os.makedirs(dump_dir, exist_ok=True)
+    np.save(os.path.join(dump_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
+
+
 class Ctx:
     """binding + (optional) torch.distributed for one bench process"""
 
@@ -373,8 +399,9 @@ class Ctx:
         return f
 
 
-def decode_leg(cx, f, hp, wtype, steps, warmup, pos0, rope, with_kernel_probe=True):
-    """-> dict of the decode figures of one model (see module docstring).  All ranks call it; figures are max-over-ranks times."""
+def decode_leg(cx, f, hp, wtype, steps, warmup, pos0, rope, with_kernel_probe=True, dump_dir=None):
+    """-> dict of the decode figures of one model (see module docstring).  All ranks call it; figures are max-over-ranks times.
+    dump_dir: the last rank writes the logits of the last timed step there (logits.npy)."""
     L, b = cx.L, cx.b
     stream = f.stream()
     tok_dev = b.DevBuf(src=np.array([1234], np.int32))
@@ -403,6 +430,10 @@ def decode_leg(cx, f, hp, wtype, steps, warmup, pos0, rope, with_kernel_probe=Tr
     wall_ms = (time.perf_counter() - t0) * 1e3
     tf_ms = L.b200_event_elapsed_ms(e0, e1)
     launches = f.last_launches() * steps
+    if dump_dir and cx.rank == cx.world - 1:
+        logits = np.empty(hp["n_vocab"], np.float32)
+        L.b200_memcpy_d2h(logits.ctypes.data_as(C.c_void_p), f.logits_dev(), logits.nbytes)
+        dump(dump_dir, "logits", logits)
 
     # ---- (2) N > 1: strict autoregressive, device-side (arg-max on the last rank, id -> rank 0 over NCCL inside the step graph)
     auto_ms = None
@@ -454,22 +485,26 @@ def decode_leg(cx, f, hp, wtype, steps, warmup, pos0, rope, with_kernel_probe=Tr
     return out
 
 
-def prompt_leg(cx, f, hp, n_tokens=2048, n_batch=512):
+def prompt_leg(cx, f, hp, n_tokens=2048, n_batch=512, repeats=1, dump_dir=None):
     """BASELINE config 3: n_tokens synthetic prompt tokens in chunks of n_batch through b200_falcon_eval (host token ids in, host logits
-    of the last token out).  N > 1: chunk c+1 enters stage 0 while chunk c is in stage 1 -- legitimate for a prompt (the KV cache of a
-    stage only depends on that stage's earlier chunks)."""
+    of the last token out), the whole prompt `repeats` times from position 0 (one timed step = one prompt).  N > 1: chunk c+1 enters
+    stage 0 while chunk c is in stage 1 -- legitimate for a prompt (the KV cache of a stage only depends on that stage's earlier chunks)."""
     toks = np.random.default_rng(7).integers(12, hp["n_vocab"], size=n_tokens).astype(np.int32)
     stream = f.stream()
     f.eval(toks[:n_batch], 0, 0)                     # warm-up (tensor maps, scratch)
     cx.barrier(stream)
     t0 = time.perf_counter()
     dev_ms = 0.0
-    for c in range(n_tokens // n_batch):
-        f.eval(toks[n_batch * c: n_batch * (c + 1)], n_batch * c, 0)
-        dev_ms += f.last_ms()
+    for _ in range(repeats):
+        for c in range(n_tokens // n_batch):
+            lg = f.eval(toks[n_batch * c: n_batch * (c + 1)], n_batch * c, 0)
+            dev_ms += f.last_ms()
     cx.barrier(stream)
+    if dump_dir and cx.rank == cx.world - 1:
+        dump(dump_dir, "prompt_logits", lg[0])
     wall_s = time.perf_counter() - t0
     wall_s, dev_ms = cx.max_over_ranks([wall_s, dev_ms])
+    wall_s, dev_ms = wall_s / repeats, dev_ms / repeats                   # per prompt
     E, H, Lh, D = hp["n_embd"], hp["n_head"], hp["n_layer"], hp["n_embd"] // hp["n_head"]
     mm_flop = 2.0 * weight_elems(hp) * n_tokens - 2.0 * E * hp["n_vocab"] * (n_tokens - n_tokens // n_batch)     # lm_head: last token of each chunk only
     att_flop = sum(4.0 * n_batch * (n_batch * c + (n_batch + 1) / 2.0) * D * H * Lh for c in range(n_tokens // n_batch))     # causal: QK^T and PV over the visible keys
@@ -480,13 +515,14 @@ def prompt_leg(cx, f, hp, n_tokens=2048, n_batch=512):
             "matmul_TFLOP": mm_flop / 1e12, "attention_TFLOP": att_flop / 1e12,
             "roofline": {"bound": "tensor", "achieved": (mm_flop + att_flop) / secs / 1e12 / cx.world, "peak": tf_peak, "unit": "TFLOP/s",
                          "frac": (mm_flop + att_flop) / secs / 1e12 / cx.world / tf_peak, "traffic": None,
-                         "what": "whole prompt (dequantising tcgen05 GEMMs + tcgen05 attention) per GPU against the sustained dense bf16 peak; "
+                         "what": "whole prompt (dequantising wgmma GEMMs + wgmma attention) per GPU against the sustained dense bf16 peak; "
                                  + ("device time (CUDA events per eval)" if cx.world == 1 else "wall clock (pipelined chunks)")},
             "roofline_tok_s": tf_peak * 1e12 * cx.world / ((mm_flop + att_flop) / n_tokens),
-            "what": "%d x b200_falcon_eval of %d host tokens; tok_s = wall clock incl. H2D / D2H" % (n_tokens // n_batch, n_batch)}
+            "repeats": repeats,
+            "what": "%d x b200_falcon_eval of %d host tokens per prompt, %d prompts; tok_s = wall clock incl. H2D / D2H" % (n_tokens // n_batch, n_batch, repeats)}
 
 
-def matvec_leg(cx, K=4096, M=4096, n_mats=32, reps=20, cpu=True):
+def matvec_leg(cx, K=4096, M=4096, n_mats=32, reps=20, cpu=True, dump_dir=None):
     """BASELINE config 1 on the GPU (+ the reference's ggml.c on the host cores): same blocks, same activation column"""
     L, b = cx.L, cx.b
     import ggllm_cpp_b200.ggcc as ggcc
@@ -510,6 +546,8 @@ def matvec_leg(cx, K=4096, M=4096, n_mats=32, reps=20, cpu=True):
     L.b200_event_record(e1, None)
     L.b200_event_synchronize(e1)
     us = L.b200_event_elapsed_ms(e0, e1) * 1e3 / (reps * n_mats)
+    if dump_dir:                                      # the timed loop's last call: the last matrix times the quantised activation
+        dump(dump_dir, "y", yd.download(np.float32, (M,)))
     # end to end: host activation column in, host result out (H2D + quantise + mat-vec + D2H), what ggml_cuda_mul_mat's caller sees
     xh, yh = np.ascontiguousarray(x[None, :]), np.zeros((1, M), np.float32)
     t0 = time.perf_counter()
@@ -523,7 +561,7 @@ def matvec_leg(cx, K=4096, M=4096, n_mats=32, reps=20, cpu=True):
     y_gpu = yd.download(np.float32, (M,))
     nbytes = K * M * 18 // 32
     peak, _, _ = peaks()
-    out = {"shape": [K, M, 1], "n_mats": n_mats, "l2": "%d rotating matrices = %.0f MB > 126 MB L2" % (n_mats, n_mats * nbytes / 1e6),
+    out = {"shape": [K, M, 1], "n_mats": n_mats, "l2": "%d rotating matrices = %.0f MB > 50 MB L2" % (n_mats, n_mats * nbytes / 1e6),
            "gpu": {"us_per_call": us, "GBs": nbytes / us / 1e3, "frac_of_hbm_peak": nbytes / us / 1e3 / peak, "GFLOPs": 2.0 * K * M / us / 1e3,
                    "e2e_us_per_call": e2e_us, "e2e_bytes": {"h2d": K * 4, "d2h": M * 4}, "roofline_us": nbytes / peak / 1e3,
                    "note": "a 9.4 MB mat-vec lasts ~2 us: back-to-back launches are launch-latency bound, not HBM bound"},
@@ -572,16 +610,17 @@ def main():
     ap.add_argument("--no-extras", action="store_true", help="only the selected config (skip the other BASELINE configs and the CPU baseline)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--layers", type=int, default=0, help="debug: fewer layers than the real model (the result is then NOT a valid bench value)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write what the timed path computed in its last step as DIR/<name>.npy")
     args = ap.parse_args()
     rank, world = int(os.environ.get("RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
     warmup = max(args.warmup, 3)
     sel = args.config
     dsel = sel if sel in DECODE_CONFIGS else "headline"
-    model, wtype, n_ctx, pos0, metric = DECODE_CONFIGS[dsel]
+    model, wtype, n_ctx, pos0, metric = decode_config(dsel, world)
     rope = 129 if pos0 == 0 else n_ctx               # falcon_main sets n_max_real_ctx = prompt + n_predict (falcon_main.cpp:835-836)
-    config = {"workload": WORKLOAD[sel] + (", STRICT AUTOREGRESSIVE (device-side arg-max feeds the next step)" if world > 1 and sel != "3" else ""),
+    config = {"workload": workload(sel, world) + (", STRICT AUTOREGRESSIVE (device-side arg-max feeds the next step)" if world > 1 and sel != "3" else ""),
               "baseline_config": sel, "model_shape": MODELS[model], "weights": TYPE_NAME[wtype], "n_ctx": n_ctx, "n_ctx_rope": rope,
-              "l2": "inputs (the weights streamed per step, GBs) are far larger than the 126 MB L2; no explicit flush needed",
+              "l2": "inputs (the weights streamed per step, GBs) are far larger than the 50 MB L2; no explicit flush needed",
               "parallelism": ("layer-range pipeline x%d (contiguous layers per GPU balanced by bytes, ncclSend/ncclRecv of the residual per boundary, "
                               "sampled id last rank -> rank 0)" % world) if world > 1 else "single GPU"}
 
@@ -616,12 +655,12 @@ def main():
     out_extra = {}
 
     if sel == "1":
-        r = matvec_leg(cx, cpu=not args.no_cpu_baseline) if cx.rank == 0 else None
+        r = matvec_leg(cx, reps=args.steps, cpu=not args.no_cpu_baseline, dump_dir=args.dump_outputs) if cx.rank == 0 else None
         if cx.rank == 0:
             print(json.dumps({"metric": "q4_0_4096x4096_matvec_us", "value": r["gpu"]["us_per_call"], "unit": "us", "n_gpus": args.gpus, "steps": args.steps, "warmup": warmup,
                               "ms_per_step": r["gpu"]["us_per_call"] / 1e3, "higher_is_better": False, "scaling": "weak", "vs_baseline": None, "dtype": "int8 x int4 block dots (dp4a)",
                               "data": "synthetic", "config": config, "e2e": {"value": r["gpu"]["e2e_us_per_call"], "unit": "us", "h2d_bytes_per_step": 4096 * 4, "d2h_bytes_per_step": 4096 * 4},
-                              "gpu_launches": 20 * 32, "roofline": {"bound": "hbm", "achieved": r["gpu"]["GBs"], "peak": peak, "unit": "GB/s", "frac": r["gpu"]["frac_of_hbm_peak"], "traffic": None},
+                              "gpu_launches": args.steps * 32, "roofline": {"bound": "hbm", "achieved": r["gpu"]["GBs"], "peak": peak, "unit": "GB/s", "frac": r["gpu"]["frac_of_hbm_peak"], "traffic": None},
                               "cpu_baseline": {"value": r["cpu"]["us_per_call"], "unit": "us", "cores": r["cpu"]["cores"], "kind": r["cpu"]["kind"], "sample": "32 rotating matrices x 8 passes"} if r["cpu"] else None,
                               "detail": r}))
         return
@@ -629,18 +668,18 @@ def main():
     n_batch = 512 if (sel in ("headline", "3") and extras or sel == "3") else 1
     sampler = ClockSampler(cx.local_rank)
     f = cx.make_model(hp, wtype, n_ctx, n_batch)
-    d = decode_leg(cx, f, hp, wtype, args.steps, warmup, pos0, rope)
+    d = decode_leg(cx, f, hp, wtype, args.steps, warmup, pos0, rope, dump_dir=args.dump_outputs if sel != "3" else None)
     clocks = sampler.stop()
     prompt = None
     if n_batch >= 512:
-        prompt = prompt_leg(cx, f, hp)
+        prompt = prompt_leg(cx, f, hp, repeats=args.steps if sel == "3" else 1, dump_dir=args.dump_outputs if sel == "3" else None)
     f.free()
     parity = pipeline_parity(cx) if cx.world > 1 else None
 
     if extras and sel == "headline":
         steps_x = max(8, min(args.steps, 64))
         for key in ("2", "4", "5"):
-            m2, wt2, nctx2, pos2, metric2 = DECODE_CONFIGS[key]
+            m2, wt2, nctx2, pos2, metric2 = decode_config(key, cx.world)
             if key == "2" and cx.world > 1:
                 continue                                  # BASELINE runs Falcon-7B on one GPU
             try:
@@ -648,7 +687,7 @@ def main():
                 r2 = decode_leg(cx, f2, MODELS[m2], wt2, 128 if key == "2" and cx.world == 1 else steps_x, warmup, pos2, 129 if pos2 == 0 else nctx2, with_kernel_probe=False)
                 f2.free()
                 r2.pop("_probe", None)
-                r2.update(metric=metric2, workload=WORKLOAD[key], steps=128 if key == "2" and cx.world == 1 else steps_x)
+                r2.update(metric=metric2, workload=workload(key, cx.world), steps=128 if key == "2" and cx.world == 1 else steps_x)
                 out_extra["cfg" + key] = r2
             except Exception as ex:                       # an extra config must never take the headline down
                 out_extra["cfg" + key] = {"error": repr(ex)}
@@ -661,18 +700,10 @@ def main():
         return
 
     mv_ms, mv_n, mv_bytes = d.pop("_probe")
-    traffic, traffic_src = None, None
-    for tname in ("r2_traffic.json", "r1_traffic.json"):          # ncu launch list of this command, summarised by tools/launch_list.py
-        try:
-            with open(os.path.join(ROOT, "profiles", tname)) as tf:
-                tj = json.load(tf)
-            traffic, traffic_src = float(tj["dram_bytes_per_matvec_launch"]), tj.get("source", tname)
-            break
-        except Exception:
-            pass
+    traffic = None                                                # DRAM bytes per launch need a hardware-counter profile: not measured
     ach = mv_bytes / (mv_ms / 1e3) / 1e9
     if sel == "3":
-        value, unit, metric_name, ms_step = prompt["tok_s"], "tok/s", "falcon40b_q4_k_prompt_tokens_per_s", prompt["seconds"] * 1e3 / 4
+        value, unit, metric_name, ms_step = prompt["tok_s"], "tok/s", "falcon40b_q4_k_prompt_tokens_per_s", prompt["seconds"] * 1e3
         e2e = {"value": prompt["tok_s"], "unit": "tok/s", "h2d_bytes_per_step": 512 * 4, "d2h_bytes_per_step": hp["n_vocab"] * 4, "api": "b200_falcon_eval (512 host token ids in, host logits out)"}
     else:
         value, unit, metric_name, ms_step = d["tok_s"], "tok/s", metric, d["ms_per_step"]
@@ -685,7 +716,6 @@ def main():
            "step_roofline_frac": d["step_frac"],
            "roofline": {"bound": "hbm", "kernel": "mmv_fast_kernel<%s> (register-resident fused dequantise + int8 dot mat-vec)" % TYPE_NAME[wtype], "achieved": ach, "peak": peak,
                         "unit": "GB/s", "frac": ach / peak, "peak_source": peak_src, "traffic": traffic,
-                        "traffic_source": ("ncu dram__bytes_read.sum + dram__bytes_write.sum per mat-vec launch: " + traffic_src) if traffic else None,
                         "launches_timed": int(mv_n), "avg_launch_us": mv_ms * 1e3 / max(mv_n, 1), "algorithmic_bytes_per_launch": mv_bytes / max(mv_n, 1),
                         "how": "all resident mat-vecs of rank 0 (4 per layer + lm_head) launched back to back x3 on the eval stream, CUDA events around the region; "
                                "each launch reads a different matrix, one pass >> L2",

@@ -1,7 +1,7 @@
 """ctypes binding of csrc/libggml_b200.so (the C ABI declared in include/ggml_b200.h).
 
 Used by tests/ and bench.py only; the library itself has no Python dependency.  There is no fallback of any
-kind: if the CUDA library is missing or no sm_100 GPU is visible, loading / init fails loudly.
+kind: if the CUDA library is missing or no sm_90 GPU is visible, loading / init fails loudly.
 """
 import ctypes as C
 import os
@@ -28,7 +28,7 @@ PART_B = ["b200_falcon_create", "b200_falcon_set_tensor", "b200_falcon_set_tenso
 
 
 def build(verbose=False):
-    """nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo for every .cu (csrc/Makefile); cross-compiles without a GPU."""
+    """nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo for every .cu (csrc/Makefile); cross-compiles without a GPU."""
     subprocess.check_call(["make", "-C", CSRC, "-j8"] + ([] if verbose else ["-s"]))
     return LIB_PATH
 

@@ -88,8 +88,8 @@ __global__ void __launch_bounds__(ATT_THREADS) attention_kernel(const float * __
 
 // ------------------------------------------------------------------------------------------------------------------
 // Split-KV decode attention (n_tok == 1, head_dim 64).  The kernel above walks a head's keys with one 128-thread CTA and
-// re-reads the KV head's K / V once per query head: fine at 100 keys, 745 us per layer at 8192 (tools/ctx_decode.py:
-// 210 tok/s at n_past 8, 20 tok/s at 8184).  Here the G query heads of a KV head are processed TOGETHER (K / V are read
+// re-reads the KV head's K / V once per query head: fine at 100 keys, far too slow at thousands
+// (tools/ctx_decode.py shows the decode rate against the context position).  Here the G query heads of a KV head are processed TOGETHER (K / V are read
 // once per KV head) and the keys are split over AT_SPLITS CTAs per KV head:
 //   kernel 1 (scores): a warp takes one key per step, lane l holds dims 2l, 2l+1 of the key (one coalesced 256-byte row) and
 //                      of the G <= 16 query vectors; G partial dots per lane are reduced with a transposing butterfly

@@ -6,17 +6,13 @@
 //     128-thread CTAs, so the 256-CTA grid of attention.cu runs as two waves of latency-bound CTAs
 //   * rows stream through a warp-private cp.async ring (AL_KR stages of AL_KB = 8 rows, padded against bank conflicts): only __syncwarp
 //     is involved and the next stage is in flight while one is consumed, without holding registers
-//   * both products run on the TENSOR CORES: the G <= 16 query heads of a KV head are exactly the M = 16 of a warp-level mma.  ncu on
-//     attention.cu's kernels at 8k keys (profiles/r2_notes.md): 151 + 119 instructions per key, one warp per scheduler, issue slots 29 %
-//     busy, no memory stall -- latency-bound instruction streams that also take issue slots from the mat-vec CTAs beside them.  A CUDA-core
-//     rewrite (lane = (key, octet), shared-memory broadcasts) reached 79 + 97; mma.sync m16n8k16 (scores) / m16n8k8 (values) with the fp32
-//     operands split into fp16 hi + lo terms reaches 24 + 39 (profiles/r2_attention_long.md): 13 + 21 us per layer alone at 8000 keys
+//   * both products run on the TENSOR CORES: the G <= 16 query heads of a KV head are exactly the M = 16 of a warp-level mma.  At 8k keys
+//     attention.cu's kernels are latency-bound instruction streams (one warp per scheduler, ~270 instructions per key) that also take
+//     issue slots from the mat-vec CTAs beside them; mma.sync m16n8k16 (scores) / m16n8k8 (values) with the fp32 operands split into
+//     fp16 hi + lo terms needs ~60 instructions per key
 //   * values: the exponentials come out directly in A-fragment layout (lane = heads gid, gid + 8 x keys 2 tig, 2 tig + 1), no separate pass,
 //     no [key][head] array, no shuffles; the scores travel through the same ring as the V rows
-// Measured (Falcon-40B Q4_K, tok/s at n_past 8 / 2000 / 8000): attention.cu 210 / 195 / 135, this file 211 / 210 / 192; Falcon-180B
-// Q4_K at 8000 on one GPU (BASELINE config 5): 38.0 -> 53.9 tok/s together with the 256 x 2 mat-vec shape for K = 14848.  Against the
-// oracle the tiny-model evals stay at the 1e-8 * S level.  Falcon-7B (one KV head, five head groups re-reading it): 631 / 598 / 308 ->
-// 634 / 607 / 500 tok/s at n_past 1100 / 2000 / 8000.  Short contexts gain nothing (and the CUDA-core one-wave version was slower there):
+// Against the oracle the tiny-model evals stay at the 1e-8 * S level.  Short contexts gain nothing:
 // launch_attention picks this path above attention_long_threshold() keys; the decode graphs of engine.cu are captured per tier.
 #include "kernels.h"
 #include "actquant.cuh"

@@ -1,31 +1,27 @@
 // attention_ws.cu -- causal grouped-query attention for a batch of N > 8 new tokens (prompt processing): warp-specialised
-// tcgen05 kernel over an fp16 shadow of the KV cache.
+// Hopper kernel (TMA + wgmma) over an fp16 shadow of the KV cache.
 //
 // Contract (libfalcon.cpp:2285-2366, ggml.c:12389-12458): scores scaled by 1/sqrt(64), the row's GLOBAL maximum subtracted before
 // the fp16-LUT exp, probabilities normalised by 1/sum.  The global maximum makes it a TWO-PASS kernel: pass 1 runs S = Q K^T on
 // the tensor cores only to find the row maxima, pass 2 recomputes each S tile, turns it into e = LUT(s - max) -- an fp16 value by
-// construction, so the fp16 A operand of the second product is EXACT -- and accumulates O += e V in tensor memory.
+// construction, so the fp16 A operand of the second product is EXACT -- and accumulates O += e V in registers.
 //
-// What changed against round 1's tcgen05 kernel (removed; profiles/r1_attention_tc.md): there all
-// 256 threads of a CTA converted K and V from fp32 and transposed V with 2-byte stores IN BOTH PASSES, then ran the softmax, then
-// one thread issued the MMAs -- three serialised phases, tensor pipe 5 % busy.  Here
 //   * K and V^T live in HBM as fp16 shadows written ONCE, by the kernel that appends a token to the fp32 cache
 //     (rope_kv_append_kernel / kv_shadow_refresh_kernel), in exactly the layouts the MMA operands want:
 //       k16  [n_ctx][n_head_kv][64]       a key row is 128 bytes = one SWIZZLE_128B row of the K-major B operand of Q K^T
 //       vt16 [n_head_kv][64][ctx_pad]     V transposed: a row of the K-major B operand of P V is 64 consecutive keys of one dim
 //   * warp 0 streams the tiles with TMA (cp.async.bulk.tensor, 3-D maps) into a 3-deep K ring and a 2-deep V^T ring
-//   * warp 1 issues every tcgen05.mma; S is double-buffered in tensor memory, so Q K^T of tile i+1 runs while the softmax warps
-//     work on tile i, and P V of tile i-1 runs behind it
-//   * warps 2..17 (four threads per query row, 32 score columns each) only do the softmax: tcgen05.ld S, e = LUT(s - max), P written
-//     as fp16 into the swizzled operand layout (double-buffered); the row sums come out of the tensor core too (a row of ones
-//     appended to V^T, accumulator column 64), so the CUDA cores never add probabilities.  Sixteen warps = four per scheduler: the
-//     softmax is what bounds the kernel (one MUFU.EX2 per score, 16 lanes / clk / SM), so its latencies have to overlap
+//   * two consumer warpgroups own 64 query rows each: S = Q K^T (wgmma m64n128k16, Q and K from shared memory) lands in registers,
+//     the softmax works on the accumulator fragment in place (a row lives in one quad of lanes), and P, packed to fp16, is the
+//     REGISTER A operand of O += P V (wgmma m64n64k16), so P never goes through shared memory.  While one warpgroup runs its
+//     softmax the other one's MMAs keep the tensor core busy.
 // One CTA = 128 query rows of one KV head (row = token * G + head_in_group: the G query heads that share the KV head are stacked,
 // a K / V tile serves all of them) x all visible keys in tiles of 128; CTAs with the most key tiles are scheduled first.
-// Tensor memory: S0 [0,128) S1 [128,256) O [256,336); shared memory 171 KB -> one CTA per SM (18 warps).
-// Precision: Q, K, V rounded to fp16, fp32 accumulation, P exact; the row sum is an fp32 sum (the CPU's is double).  Tolerance:
-// tests/test_kernels_gpu.py::test_attention (atol 5e-3, median 5e-4), logits inside the GEMM-path bound.
+// Shared memory 97 KB.
+// Precision: Q, K, V rounded to fp16, fp32 accumulation, P exact; the row sum is an fp32 sum of the fp16 probabilities (the CPU's is
+// double).  Tolerance: tests/test_kernels_gpu.py::test_attention (atol 5e-3, median 5e-4), logits inside the GEMM-path bound.
 #include "kernels.h"
+#include "wgmma.cuh"
 #include <cuda.h>
 #include <cudaTypedefs.h>
 
@@ -33,54 +29,22 @@ namespace {
 
 constexpr int M = 128, NK = 128, D = 64;
 constexpr int KST = 3, VST = 2;
-constexpr int V_SUB = 10240;                        // one 64-key half of a V^T stage: 64 dims x 128 B from TMA + 16 rows (ones, zeros) = 80 rows
+constexpr int V_SUB = 8192;                         // one 64-key half of a V^T stage: 64 dims x 128 B
 constexpr int V_STAGE = 2 * V_SUB;
-constexpr int SQ = 0, SK = 16384, SV = SK + KST * 16384, SP = SV + VST * V_STAGE, SBAR = SP + 2 * 32768, SX = SBAR + 256;
-constexpr size_t SMEM_BYTES = 1024 + SX + 4 * 128 * 4;
-constexpr int N_O = 80;                             // accumulator columns of P V: 64 dims + the ones row (row sum) + 15 unused
-constexpr int SOFTMAX_THREADS = 512, THREADS = 64 + SOFTMAX_THREADS;
-constexpr uint32_t TM_S = 0, TM_O = 256, TM_COLS = 512;
+constexpr int SQ = 0, SK = 16384, SV = SK + KST * 16384, SBAR = SV + VST * V_STAGE;
+constexpr size_t SMEM_BYTES = 1024 + SBAR + 256;
+constexpr int THREADS = 384;                        // warpgroup 0: TMA (warp 0); warpgroups 1, 2: MMA + softmax
 
 __device__ __forceinline__ void mbar_arrive(uint64_t * bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(smem_u32(bar)) : "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t * bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_c, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                 :: "r"(tmem_c), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
 __device__ __forceinline__ void tma_load_3d(void * smem_dst, const CUtensorMap * map, int c0, int c1, int c2, uint64_t * bar) {
     asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                  :: "r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-// K-major, SWIZZLE_128B shared-memory matrix descriptor: rows of 128 B, 8-row groups 1024 B apart (as gemm_tc.cu)
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t) ((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t) 1 << 16;
-    d |= (uint64_t) (1024 >> 4) << 32;
-    d |= (uint64_t) 1 << 46;
-    d |= (uint64_t) 2 << 61;
-    return d;
-}
-__device__ __forceinline__ uint32_t instr_desc_f16(int n) { return (1u << 4) | ((uint32_t) (n >> 3) << 17) | ((uint32_t) (M >> 4) << 24); }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]),
-                   "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                   "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
     const __half2 h = __floats2half2_rn(a, b);
     return *reinterpret_cast<const uint32_t *>(&h);
 }
-__device__ __forceinline__ void softmax_sync() { asm volatile("bar.sync 1, %0;" :: "n"(SOFTMAX_THREADS) : "memory"); }
 // e^x for x <= 0 as the LUT computes it up to the final fp16 rounding: ex2.approx.ftz (2 ulp fp32); results below 2^-126 flush to zero,
 // which the fp16 rounding would do anyway (the plain __expf wraps the same instruction in denormal rescaling: 3 extra instructions)
 __device__ __forceinline__ float exp_fast(float x) {
@@ -111,67 +75,26 @@ __device__ __forceinline__ void store_quarter_row_f16(uint8_t * tile, int r, con
     }
 }
 
-// one 32-column slice of an S tile -> P (fp16) in the A-operand layout.  MASKED: keys >= vis are zeroed (tiles on the causal diagonal)
-template <bool MASKED>
-__device__ __forceinline__ void softmax_slice(const uint32_t (&v)[32], uint8_t * prow, int c, int t, float scale, float neg_m, int key0, int vis) {
-#pragma unroll
-    for (int q = 0; q < 4; q++) {
-        uint32_t pk[4];
-#pragma unroll
-        for (int jj = 0; jj < 4; jj++) {
-            // s - max with ONE rounding: the product with 0.125 is exact, so fma(s, 0.125, -max) == (s * 0.125) - max
-            const float x0 = __fmaf_rn(__uint_as_float(v[8 * q + 2 * jj]), scale, neg_m), x1 = __fmaf_rn(__uint_as_float(v[8 * q + 2 * jj + 1]), scale, neg_m);
-            const float2 xr = __half22float2(__floats2half2_rn(x0, x1));               // the LUT index: f16(s - max)
-            float e0 = exp_fast(xr.x), e1 = exp_fast(xr.y);
-            if (MASKED) { const int key = key0 + 8 * q + 2 * jj; if (key >= vis) e0 = 0.f; if (key + 1 >= vis) e1 = 0.f; }
-            pk[jj] = pack_h2(e0, e1);                                                   // table_exp_f16 value: exact as fp16
-        }
-        const int ci = (c & 1) * 4 + q;
-        *reinterpret_cast<uint4 *>(prow + ((ci ^ (t & 7)) << 4)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-    }
-}
-
 __global__ void __launch_bounds__(THREADS, 1) attention_ws_kernel(const __grid_constant__ CUtensorMap kmap, const __grid_constant__ CUtensorMap vmap, const WsArgs a) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t * smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t) 1023);
     uint64_t * bars = reinterpret_cast<uint64_t *>(smem + SBAR);
-    uint64_t * q_full = bars, * k_full = bars + 1, * k_empty = k_full + KST, * v_full = k_empty + KST, * v_empty = v_full + VST,
-             * s_full = v_empty + VST, * s_free = s_full + 2, * p_full = s_free + 2, * p_free = p_full + 2, * o_full = p_free + 2;
-    uint32_t * tmem_slot = reinterpret_cast<uint32_t *>(o_full + 1);
-    float * xch = reinterpret_cast<float *>(smem + SX);                   // [2][128]: exchange between the two column halves of a row
+    uint64_t * k_full = bars, * k_empty = k_full + KST, * v_full = k_empty + KST, * v_empty = v_full + VST;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int g = blockIdx.y, r0 = ((int) gridDim.x - 1 - (int) blockIdx.x) * M;      // latest rows (most key tiles) first
     const int t_last = (min(r0 + M, a.rows) - 1) / a.G;
     const int kmax = a.n_past + t_last + 1, nt = (kmax + NK - 1) / NK;
 
     if (threadIdx.x == 0) {
-        mbar_init(q_full, SOFTMAX_THREADS);
-        for (int s = 0; s < KST; s++) { mbar_init(k_full + s, 1); mbar_init(k_empty + s, 1); }
-        for (int s = 0; s < VST; s++) { mbar_init(v_full + s, 1); mbar_init(v_empty + s, 1); }
-        for (int s = 0; s < 2; s++) { mbar_init(s_full + s, 1); mbar_init(s_free + s, SOFTMAX_THREADS); mbar_init(p_full + s, SOFTMAX_THREADS); mbar_init(p_free + s, 1); }
-        mbar_init(o_full, 1);
+        for (int s = 0; s < KST; s++) { mbar_init(k_full + s, 1); mbar_init(k_empty + s, 8); }      // empty: one arrival per consumer warp
+        for (int s = 0; s < VST; s++) { mbar_init(v_full + s, 1); mbar_init(v_empty + s, 8); }
         mbar_fence_init();
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(tmem_slot)), "r"(TM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    // rows 64..79 of every V^T half-stage: row 64 = ones (the accumulator's column 64 becomes the row sum of P), rows 65..79 = zeros.
-    // A constant row is the same under the 128-byte swizzle; TMA only ever writes rows 0..63.
-    for (int i = threadIdx.x; i < VST * 2 * 16 * 8; i += THREADS) {
-        const int sub = i / (16 * 8), r = (i / 8) % 16, c = i % 8;
-        const uint32_t one2 = 0x3C003C00u;                                 // two fp16 1.0
-        *reinterpret_cast<uint4 *>(smem + SV + sub * V_SUB + (64 + r) * 128 + c * 16) = r == 0 ? make_uint4(one2, one2, one2, one2) : make_uint4(0, 0, 0, 0);
-    }
-    fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp < 4) {
         // ================================================================ TMA producer
-        if (lane == 0) {
+        if (warp == 0 && lane == 0) {
             for (int j = 0; j < 2 * nt; j++) {
                 const int kt = j < nt ? j : j - nt, s = j % KST;
                 if (j >= KST) mbar_wait(k_empty + s, (uint32_t) ((j / KST - 1) & 1));
@@ -186,117 +109,112 @@ __global__ void __launch_bounds__(THREADS, 1) attention_ws_kernel(const __grid_c
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================================================================ MMA issuer
-        if (lane == 0) {
-            const uint32_t q_addr = smem_u32(smem + SQ), id_s = instr_desc_f16(NK), id_o = instr_desc_f16(N_O);
-            auto pv = [&](int i) {                                          // O += P_i V_i
-                const int b = i & 1;
-                mbar_wait(p_full + b, (uint32_t) ((i >> 1) & 1));
-                mbar_wait(v_full + b, (uint32_t) ((i >> 1) & 1));
-                tc_fence_after();
-                const uint32_t p_addr = smem_u32(smem + SP + b * 32768), v_addr = smem_u32(smem + SV + b * V_STAGE);
-#pragma unroll
-                for (int k = 0; k < NK / 16; k++)
-                    tc_mma_f16(tmem_base + TM_O, umma_desc(p_addr + (k >> 2) * 16384 + (k & 3) * 32), umma_desc(v_addr + (k >> 2) * V_SUB + (k & 3) * 32), id_o, (i | k) != 0);
-                tc_commit(p_free + b);
-                tc_commit(v_empty + b);
-            };
-            mbar_wait(q_full, 0);
-            for (int j = 0; j < 2 * nt; j++) {
-                const int s = j % KST, b = j & 1;
-                mbar_wait(k_full + s, (uint32_t) ((j / KST) & 1));
-                if (j >= 2) mbar_wait(s_free + b, (uint32_t) (((j >> 1) - 1) & 1));
-                tc_fence_after();
-                const uint32_t k_addr = smem_u32(smem + SK + s * 16384);
-#pragma unroll
-                for (int k = 0; k < D / 16; k++) tc_mma_f16(tmem_base + TM_S + b * NK, umma_desc(q_addr + k * 32), umma_desc(k_addr + k * 32), id_s, k != 0);
-                tc_commit(k_empty + s);
-                tc_commit(s_full + b);
-                if (j >= nt + 1) pv(j - nt - 1);                            // behind the NEXT tile's Q K^T, so the softmax of tile i overlaps both
-            }
-            pv(nt - 1);
-            tc_commit(o_full);
-        }
-    } else {
-        // ================================================================ softmax warps: thread = (row t, 32-column slice c)
-        const int q4 = warp & 3, c = (warp - 2) >> 2, t = q4 * 32 + lane;   // a warp may only touch TMEM lanes 32 (warp % 4) ..
-        const int row = r0 + t;
-        const bool row_ok = row < a.rows;
-        const int tok = row / a.G, head = g * a.G + row % a.G;
-        const int vis = row_ok ? a.n_past + tok + 1 : 0;                    // causal: keys < vis (ggml.c:12342-12348)
-        const int vis_min = r0 + M <= a.rows ? a.n_past + r0 / a.G + 1 : 0; // keys visible to EVERY row of the tile (0 if it has padding rows)
-        const float scale = 0.125f;                                         // 1 / sqrt(64), a power of two: s * scale is exact
-        const uint32_t tm_lane = tmem_base + ((uint32_t) (q4 * 32) << 16);
-        store_quarter_row_f16(smem + SQ, t, a.qkv + (size_t) tok * a.qkv_stride + (size_t) head * D, row_ok, c);
-        fence_proxy_async();
-        mbar_arrive(q_full);
+        return;
+    }
 
-        // ---- pass 1: the row maximum of the raw scores (scale > 0: max(scale * s) = scale * max(s))
-        float mraw = -INFINITY;
-        for (int kt = 0; kt < nt; kt++) {
-            const int b = kt & 1, k0 = kt * NK;
-            mbar_wait(s_full + b, (uint32_t) ((kt >> 1) & 1));
-            tc_fence_after();
-            uint32_t v[32];
-            tmem_ld32(tm_lane + TM_S + b * NK + c * 32, v);
-            tc_fence_before();
-            mbar_arrive(s_free + b);                                        // the scores are in registers: the tensor core may overwrite the buffer
-            if (k0 + NK <= vis_min) {
+    // ==================================================================== consumer warpgroup wg = 0, 1: query rows [64 wg, +64) of the tile
+    const int ct = threadIdx.x - 128, wg = ct >> 7, wq = (ct >> 5) & 3;
+    {   // Q tile: two threads per row, 32 values each, fp32 -> fp16 into the swizzled A-operand layout
+        const int t = ct >> 1, row = r0 + t;
+        const bool ok = row < a.rows;
+        const float * src = a.qkv + (size_t) (ok ? row / a.G : 0) * a.qkv_stride + (size_t) (g * a.G + (ok ? row % a.G : 0)) * D;
+        store_quarter_row_f16(smem + SQ, t, src, ok, 2 * (ct & 1));
+        store_quarter_row_f16(smem + SQ, t, src, ok, 2 * (ct & 1) + 1);
+        fence_proxy_async();                                                // generic-proxy stores -> visible to the tensor core
+        asm volatile("bar.sync %0, 128;" :: "r"(1 + wg) : "memory");        // this warpgroup's 64 rows are written
+    }
+    // this thread's two rows of the accumulator fragments: i = 0, 1 -> tile row 64 wg + 16 wq + lane / 4 + 8 i
+    int tok[2], head[2], vis[2];
+    bool row_ok[2];
 #pragma unroll
-                for (int j = 0; j < 32; j++) mraw = fmaxf(mraw, __uint_as_float(v[j]));
-            } else {
-#pragma unroll
-                for (int j = 0; j < 32; j++) if (k0 + c * 32 + j < vis) mraw = fmaxf(mraw, __uint_as_float(v[j]));
-            }
-        }
-        xch[c * 128 + t] = mraw;
-        softmax_sync();
-        const float m = __fmul_rn(fmaxf(fmaxf(xch[t], xch[128 + t]), fmaxf(xch[256 + t], xch[384 + t])), scale);
-        const float neg_m = -m;
+    for (int i = 0; i < 2; i++) {
+        const int row = r0 + 64 * wg + 16 * wq + (lane >> 2) + 8 * i;
+        row_ok[i] = row < a.rows;
+        tok[i] = row / a.G; head[i] = g * a.G + row % a.G;
+        vis[i] = row_ok[i] ? a.n_past + tok[i] + 1 : 0;                     // causal: keys < vis (ggml.c:12342-12348)
+    }
+    const int vis_min = r0 + M <= a.rows ? a.n_past + r0 / a.G + 1 : 0;     // keys visible to EVERY row of the tile (0 if it has padding rows)
+    const float scale = 0.125f;                                             // 1 / sqrt(64), a power of two: s * scale is exact
+    const int col = 2 * (lane & 3);                                         // column of fragment element 4 c + 2 i + e: 8 c + col + e
+    const uint32_t q_addr = smem_u32(smem + SQ) + wg * 64 * 128;
 
-        // ---- pass 2: e = table_exp_f16[f16(s - max)] (ggml.c:12427-12440), P = e as fp16 (exact), written into the A operand layout
-        for (int i = 0; i < nt; i++) {
-            const int j = nt + i, b = j & 1, pb = i & 1, k0 = i * NK;
-            mbar_wait(s_full + b, (uint32_t) ((j >> 1) & 1));
-            tc_fence_after();
-            uint32_t v[32];
-            tmem_ld32(tm_lane + TM_S + b * NK + c * 32, v);
-            tc_fence_before();
-            mbar_arrive(s_free + b);
-            if (i >= 2) mbar_wait(p_free + pb, (uint32_t) (((i >> 1) - 1) & 1));
-            uint8_t * prow = smem + SP + pb * 32768 + (c >> 1) * 16384 + t * 128;
-            if (k0 + NK <= vis_min) softmax_slice<false>(v, prow, c, t, scale, neg_m, 0, 0);
-            else softmax_slice<true>(v, prow, c, t, scale, neg_m, k0 + c * 32, vis);
-            fence_proxy_async();                                            // P: generic-proxy stores -> visible to the tensor core
-            mbar_arrive(p_full + pb);
-        }
-
-        // ---- epilogue: O / sum -> out[tok][head * 64 + ...]: slice c of the row writes dims 16 c .. 16 c + 15
-        mbar_wait(o_full, 0);
-        tc_fence_after();
-        {
-            uint32_t v[32];
-            tmem_ld32(tm_lane + TM_O + 48, v);                              // columns 48..79: v[16] = column 64 = sum of the row's P (ones row of V^T)
-            const float l = __uint_as_float(v[16]);
-            const float inv = (float) (1.0 / (double) l);                   // ggml.c:12427-12449
-            uint32_t o[32];
-            tmem_ld32(tm_lane + TM_O + (c >> 1) * 32, o);                   // warp-collective: every lane loads, valid rows store
-            float * dst = a.out + (size_t) tok * a.out_stride + (size_t) head * D + c * 16;
-            if (row_ok) {
+    float mraw[2] = { -INFINITY, -INFINITY }, neg_m[2] = { 0.f, 0.f }, lsum[2] = { 0.f, 0.f };
+    float o[32];
 #pragma unroll
-                for (int jj = 0; jj < 16; jj += 4) {                        // (compile-time register indices: no local-memory array)
-                    const float4 lo = make_float4(__uint_as_float(o[jj]), __uint_as_float(o[jj + 1]), __uint_as_float(o[jj + 2]), __uint_as_float(o[jj + 3]));
-                    const float4 hi = make_float4(__uint_as_float(o[16 + jj]), __uint_as_float(o[17 + jj]), __uint_as_float(o[18 + jj]), __uint_as_float(o[19 + jj]));
-                    const float4 x = (c & 1) ? hi : lo;
-                    *reinterpret_cast<float4 *>(dst + jj) = make_float4(__fmul_rn(x.x, inv), __fmul_rn(x.y, inv), __fmul_rn(x.z, inv), __fmul_rn(x.w, inv));
+    for (int i = 0; i < 32; i++) o[i] = 0.f;
+    for (int j = 0; j < 2 * nt; j++) {
+        const int s = j % KST, kt = j < nt ? j : j - nt, k0 = kt * NK;
+        mbar_wait(k_full + s, (uint32_t) ((j / KST) & 1));
+        float sc[64];
+        const uint32_t k_addr = smem_u32(smem + SK + s * 16384);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < D / 16; k++) Wgmma<128>::mma(sc, wgmma_desc(q_addr + k * 32), wgmma_desc(k_addr + k * 32), k != 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(sc);
+        if (lane == 0) mbar_arrive(k_empty + s);                            // the scores are in registers: the K stage may be refilled
+        const bool full = k0 + NK <= vis_min;
+        if (j < nt) {
+            // ---- pass 1: the row maximum of the raw scores (scale > 0: max(scale * s) = scale * max(s))
+#pragma unroll
+            for (int c = 0; c < 16; c++)
+#pragma unroll
+                for (int i = 0; i < 2; i++)
+#pragma unroll
+                    for (int e = 0; e < 2; e++)
+                        if (full || k0 + 8 * c + col + e < vis[i]) mraw[i] = fmaxf(mraw[i], sc[4 * c + 2 * i + e]);
+            if (j == nt - 1) {
+#pragma unroll
+                for (int i = 0; i < 2; i++) {
+                    float m = fmaxf(mraw[i], __shfl_xor_sync(0xffffffffu, mraw[i], 1));
+                    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+                    neg_m[i] = -__fmul_rn(m, scale);
                 }
             }
+            continue;
         }
+        // ---- pass 2: e = table_exp_f16[f16(s - max)] (ggml.c:12427-12440), P = e as fp16 (exact), packed into the A fragments of P V
+        uint32_t p[8][4];
+#pragma unroll
+        for (int c = 0; c < 16; c++)
+#pragma unroll
+            for (int i = 0; i < 2; i++) {
+                // s - max with ONE rounding: the product with 0.125 is exact, so fma(s, 0.125, -max) == (s * 0.125) - max
+                const float x0 = __fmaf_rn(sc[4 * c + 2 * i], scale, neg_m[i]), x1 = __fmaf_rn(sc[4 * c + 2 * i + 1], scale, neg_m[i]);
+                const float2 xr = __half22float2(__floats2half2_rn(x0, x1));   // the LUT index: f16(s - max)
+                float e0 = exp_fast(xr.x), e1 = exp_fast(xr.y);
+                if (!full) { const int key = k0 + 8 * c + col; if (key >= vis[i]) e0 = 0.f; if (key + 1 >= vis[i]) e1 = 0.f; }
+                const uint32_t pk = pack_h2(e0, e1);                         // table_exp_f16 value: exact as fp16
+                const float2 ef = __half22float2(*reinterpret_cast<const __half2 *>(&pk));
+                lsum[i] += ef.x + ef.y;
+                p[c >> 1][(c & 1) * 2 + i] = pk;
+            }
+        const int i = j - nt, vs = i % VST;
+        mbar_wait(v_full + vs, (uint32_t) ((i / VST) & 1));
+        const uint32_t v_addr = smem_u32(smem + SV + vs * V_STAGE);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < NK / 16; kk++) wgmma_rs_n64(o, p[kk], wgmma_desc(v_addr + (kk >> 2) * V_SUB + (kk & 3) * 32));
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(o);
+        if (lane == 0) mbar_arrive(v_empty + vs);
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "r"(TM_COLS) : "memory");
+
+    // ---- epilogue: O / sum -> out[tok][head * 64 + ...]
+#pragma unroll
+    for (int i = 0; i < 2; i++) {
+        float l = lsum[i];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        const float inv = (float) (1.0 / (double) l);                       // ggml.c:12427-12449
+        if (!row_ok[i]) continue;
+        float * dst = a.out + (size_t) tok[i] * a.out_stride + (size_t) head[i] * D + col;
+#pragma unroll
+        for (int c = 0; c < 8; c++)
+            *reinterpret_cast<float2 *>(dst + 8 * c) = make_float2(__fmul_rn(o[4 * c + 2 * i], inv), __fmul_rn(o[4 * c + 2 * i + 1], inv));
+    }
 }
 
 PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
@@ -334,7 +252,7 @@ size_t attention_shadow_halves(int n_head_kv, int n_ctx) { return (size_t) n_hea
 void launch_kv_shadow_refresh(const float * k_cache, const float * v_cache, __half * k16, __half * vt16, int n_head_kv, int n_ctx, int pos, int n, cudaStream_t stream) {
     if (n <= 0) return;
     const int64_t total = (int64_t) n * n_head_kv * 64;
-    const unsigned grid = (unsigned) (total / 256 + 1 > 148 * 8 ? 148 * 8 : total / 256 + 1);
+    const unsigned grid = (unsigned) (total / 256 + 1 > 132 * 8 ? 132 * 8 : total / 256 + 1);
     kv_shadow_refresh_kernel<<<grid, 256, 0, stream>>>(k_cache, v_cache, k16, vt16, n_head_kv, attention_ctx_pad(n_ctx), pos, n);
     B200_CUDA_CHECK(cudaGetLastError());
 }

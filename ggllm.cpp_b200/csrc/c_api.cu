@@ -63,7 +63,7 @@ int b200_init(int device) {
     int sms = 0, major = 0;
     B200_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
     B200_CUDA_CHECK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-    if (major != 10) { fprintf(stderr, "b200: device %d has compute capability %d.x; this library is sm_100a only\n", device, major); exit(1); }
+    if (major != 9) { fprintf(stderr, "b200: device %d has compute capability %d.x; this library is built for sm_90a (H100) only\n", device, major); exit(1); }
     return sms;
 }
 
@@ -203,7 +203,7 @@ void b200_attention(float * qkv, float * kc, float * vc, float * out, int n_head
     AttnParams p = { n_head, n_head_kv, head_dim, n_tok, n_past, nullptr, n_ctx, (int64_t) (n_head + 2 * n_head_kv) * head_dim, nullptr };
     launch_rope_kv_append(qkv, kc, vc, p, rope_theta_scale_host(head_dim, n_ctx_rope ? n_ctx_rope : n_ctx, 1, 2.0f, 0), g_stream);   // libfalcon.cpp:2231-2234
     if (n_tok > 1) {
-        // the warp-specialised tcgen05 kernel reads an fp16 shadow of the cache: built here from the caller's fp32 cache (the engine
+        // the warp-specialised wgmma kernel reads an fp16 shadow of the cache: built here from the caller's fp32 cache (the engine
         // keeps one up to date token by token instead)
         static __half * sh = nullptr; static size_t sh_halves = 0;
         const size_t need = head_dim == 64 ? attention_shadow_halves(n_head_kv, n_ctx) : 0;

@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host helpers for the sm_100a backend.
+// common.cuh -- shared device/host helpers for the sm_90a (H100) backend.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -36,7 +36,7 @@ static inline size_t round_up(size_t v, size_t a) { return (v + a - 1) / a * a; 
 
 // One L1/shared-memory split (percent of shared) for every kernel of the decode step.  An SM cannot host kernels that
 // ask for different carve-outs at the same time, so without this the small attention kernels wait for the big
-// mat-vec of the other stream to drain (measured, profiles/r1_decode_timeline.md).  25 % = 57 KB shared, rest L1.
+// mat-vec of the other stream to drain.  25 % of the H100's 228 KB = 57 KB shared, rest L1.
 #define B200_CARVEOUT 25
 
 #ifdef __CUDACC__

@@ -631,7 +631,7 @@ static void enqueue_decode_fused(b200_falcon * f, int n_past, float theta_scale,
         B200_CUDA_CHECK(cudaEventRecord(f->e_join, sb));
         if (!skip("up")) launch_mmv(L.up, xm, f->up, f->FF, gelu, sa);                                           // :2389-2392
         // The attention kernels of the side stream run BESIDE ffn_up, and beside ffn_down too when its CTAs leave them registers
-        // (Falcon-40B / 180B: at long contexts the attention outlasts ffn_up, 132 tok/s at 8k that way against 109 with wo first).
+        // (Falcon-40B / 180B: at long contexts the attention outlasts ffn_up, and this order beat wo first).
         // Falcon-7B's ffn_down shape fills the SMs: attention work still pending when ffn_up ends would be shut out until it had
         // drained, so there wo (which has to wait for the attention anyway) goes first.
         const bool wo_first = mmv_fast_fills_sm(L.down);

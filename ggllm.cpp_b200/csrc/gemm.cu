@@ -6,7 +6,7 @@ bool launch_gemm_tc(const WPlanes & W, const __half * X, int64_t x_stride, int N
 
 size_t mmq_gemm_workspace_bytes(const WPlanes &, int) { return 256; }
 
-// tcgen05 kernel in chunks of <= 512 tokens (the accumulator columns one CTA owns in TMEM); shapes it does not cover
+// wgmma kernel in chunks of <= 512 tokens (it tiles the tokens by up to 256 per CTA); shapes it does not cover
 // (K not a multiple of 64) go to the CUDA-core kernel
 void launch_mmq_gemm(const WPlanes & W, const __half * X, int64_t x_stride, int N, float * Y, int64_t y_stride,
                      int epi_gelu, void *, size_t, cudaStream_t stream) {

@@ -1,7 +1,7 @@
 // gemm_simt.cu -- plain CUDA-core tiled GEMM with on-the-fly dequantisation.
 //
 // NOT the product path for the prompt mat-mat: it exists (a) as the first correct implementation of
-// Y[n][m] = sum_k fp16(W[m][k]) * X_f16[n][k] against which the tcgen05 kernel (gemm_tc.cu) is bit-compared in the
+// Y[n][m] = sum_k fp16(W[m][k]) * X_f16[n][k] against which the wgmma kernel (gemm_tc.cu) is bit-compared in the
 // tests, and (b) as the N-tail handler for shapes the tensor-core tiling does not cover.  Same operand rounding
 // as the tensor-core kernel: weights dequantised bit-exactly to fp32 then rounded once to fp16, activations fp16,
 // fp32 accumulation.

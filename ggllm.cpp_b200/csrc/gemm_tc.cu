@@ -1,70 +1,39 @@
-// gemm_tc.cu -- prompt mat-mat on the 5th-generation tensor cores: Y[n][m] = sum_k fp16(W[m][k]) * X[n][k].
+// gemm_tc.cu -- prompt mat-mat on the Hopper tensor cores (wgmma): Y[n][m] = sum_k fp16(W[m][k]) * X[n][k].
 //
 // Replaces the reference's prompt path (ggml-cuda.cu:2353-2403): dequantise the WHOLE weight matrix to an fp16
 // temporary (to_fp16_cuda, 2 B/weight written and re-read = 4.6x the quantised bytes), convert activations
 // (float_to_half + stream sync), cublasGemmEx, per call.  Here the quantised blocks are the only thing read from
-// HBM; a tile is dequantised once, straight into the shared-memory operand layout of tcgen05.mma, and used for every
-// token of the batch (up to 512 accumulator columns live in TMEM).
+// HBM; a tile is dequantised once, straight into the shared-memory operand layout of wgmma, and used for BN tokens.
 //
-// One CTA = one 128-row tile of W over the full K and ALL N tokens (N <= 512):
-//   warp 0      : TMA producer of the activation tile  B[N x 64] fp16 (cp.async.bulk.tensor.2d, SWIZZLE_128B), ring of SB stages
-//   warp 1      : allocates TMEM (512 columns), single elected thread issues tcgen05.mma.cta_group::1.kind::f16
-//                 (M = 128, N <= 256 per instruction, K = 16), tcgen05.commit releases the smem stages
-//   warps 2..17 : dequant producers: 4 threads per weight row, 16 weights each per 64-wide K block, written as
-//                 8 halves per 16-byte chunk into the K-major SWIZZLE_128B layout (chunk c of row r at c ^ (r & 7)),
-//                 fence.proxy.async, mbarrier arrive; ring of SA stages.  After the main loop the same warps are the
-//                 epilogue: tcgen05.ld 32x32b.x32 -> (GELU) -> coalesced fp32 stores.
-// Operands: A = weights (K-major smem), B = activations (K-major smem), D = fp32 in TMEM, lane = weight row.
+// One CTA = one 128-row tile of W x one tile of BN <= 256 tokens (BN = 64, 128 or 256: the accumulator lives in registers,
+// 64 x BN fp32 per consumer warpgroup) over its share of K:
+//   warpgroup 0    : dequant producers, one thread per weight row, 64 weights per 64-wide K block written as 8 halves per
+//                    16-byte chunk into the K-major SWIZZLE_128B layout (chunk c of row r at c ^ (r & 7)), fence.proxy.async,
+//                    mbarrier arrive; thread 0 also streams the activation tile B[BN x 64] fp16 with TMA
+//                    (cp.async.bulk.tensor.2d, SWIZZLE_128B).  Ring of ST stages, A and B of a stage released together.
+//   warpgroups 1, 2: wgmma.mma_async m64nBNk16, rows [64 (g - 1), +64) of the tile, both operands from shared memory; one
+//                    wgmma group stays in flight while the next stage is awaited.  Epilogue straight from the accumulator
+//                    registers: (GELU) -> fp32 stores.
+// Token tiles of the same weight tile are neighbours in the grid (blockIdx.x), so their quantised blocks come from L2.
 #include "kernels.h"
+#include "wgmma.cuh"
 #include <cuda.h>
 #include <cudaTypedefs.h>
 
 namespace {
 
-constexpr int BM = 128, BK = 64, SA = 4, SB = 2;
+constexpr int BM = 128, BK = 64, ST = 4;
 constexpr int N_MAX = 512;
-constexpr int PRODUCER_THREADS = 512, THREADS = 64 + PRODUCER_THREADS;      // 4 threads per weight row: the dequantisation is a chain of dependent
-                                                                            // fp32 ops per weight, 16 warps hide its latency (8 warps: 1.0 PFLOP/s)
+constexpr int THREADS = 384;                               // producer warpgroup + two consumer warpgroups
 constexpr int A_STAGE = BM * BK * 2;                       // 16 KB
 
 __device__ __forceinline__ void mbar_arrive(uint64_t * bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t * bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_c, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                 :: "r"(tmem_c), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
 __device__ __forceinline__ void tma_load_2d(void * smem_dst, const CUtensorMap * map, int c0, int c1, uint64_t * bar) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                  :: "r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
-}
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): 8-row groups 1024 B apart
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t) ((smem_addr & 0x3FFFF) >> 4);           // start address, 16-byte units
-    d |= (uint64_t) 1 << 16;                                // leading byte offset (unused for swizzled K-major)
-    d |= (uint64_t) (1024 >> 4) << 32;                      // stride byte offset between 8-row groups
-    d |= (uint64_t) 1 << 46;                                // descriptor version (Blackwell)
-    d |= (uint64_t) 2 << 61;                                // SWIZZLE_128B
-    return d;
-}
-__device__ __forceinline__ uint32_t instr_desc_f16(int n) {  // cute::UMMA::InstrDescriptor: f16 x f16 -> f32, both K-major, M = 128
-    return (1u << 4) | ((uint32_t) (n >> 3) << 17) | ((uint32_t) (BM >> 4) << 24);
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]),
-                   "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                   "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
     const __half2 h = __floats2half2_rn(a, b);
@@ -222,316 +191,114 @@ template <> struct Prod<T_Q3_K> {
 struct GemmArgs {
     WPlanes W;
     float * Y; int64_t y_stride;
-    int N, NT;            // tokens; tokens rounded up to 16 (accumulator columns used)
-    int box_rows;         // rows of one TMA box of the activation tile (<= 256)
+    int N;                // tokens
     int epi_gelu;
-    int ksplit;           // K is split over gridDim.y CTAs; > 1: partial tiles are added into a zeroed Y with atomics
+    int ksplit;           // K is split over gridDim.z CTAs; > 1: partial tiles are added into a zeroed Y with atomics
                           // (ksplit == 2 keeps the result deterministic: 0 + a + b is the same in either order)
 };
 
-template <int TYPE>
+template <int TYPE, int BN>
 __global__ void __launch_bounds__(THREADS, 1) gemm_tc_kernel(const __grid_constant__ CUtensorMap xmap, const GemmArgs a) {
+    constexpr int B_STAGE = BN * 128;                                      // BN token rows of 64 halves
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t * smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t) 1023);
-    const int b_stage = a.box_rows * (a.NT > 256 ? 2 : 1) * 128;          // bytes of one activation stage
-    uint8_t * sA = smem;                                                   // SA stages of 16 KB
-    uint8_t * sB = smem + SA * A_STAGE;                                    // SB stages
-    uint64_t * bars = reinterpret_cast<uint64_t *>(sB + SB * b_stage);
-    uint64_t * a_full = bars, * a_empty = bars + SA, * b_full = bars + 2 * SA, * b_empty = bars + 2 * SA + SB, * acc_full = bars + 2 * SA + 2 * SB;
-    uint32_t * tmem_slot = reinterpret_cast<uint32_t *>(acc_full + 1);
+    uint8_t * sA = smem;                                                   // ST stages of 16 KB
+    uint8_t * sB = smem + ST * A_STAGE;                                    // ST stages of BN x 128 B
+    uint64_t * bars = reinterpret_cast<uint64_t *>(sB + ST * B_STAGE);
+    uint64_t * a_full = bars, * b_full = bars + ST, * empty = bars + 2 * ST;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int m0 = blockIdx.x * BM;
+    const int n0 = blockIdx.x * BN, m0 = blockIdx.y * BM;
     const int KBT = a.W.K / BK;                                            // K blocks in total; this CTA owns [kb0, kb0 + KB)
-    const int kb0 = (int) ((int64_t) KBT * blockIdx.y / a.ksplit), KB = (int) ((int64_t) KBT * (blockIdx.y + 1) / a.ksplit) - kb0;
+    const int kb0 = (int) ((int64_t) KBT * blockIdx.z / a.ksplit), KB = (int) ((int64_t) KBT * (blockIdx.z + 1) / a.ksplit) - kb0;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < SA; s++) { mbar_init(a_full + s, PRODUCER_THREADS); mbar_init(a_empty + s, 1); }
-        for (int s = 0; s < SB; s++) { mbar_init(b_full + s, 1); mbar_init(b_empty + s, 1); }
-        mbar_init(acc_full, 1);
+        for (int s = 0; s < ST; s++) { mbar_init(a_full + s, 128); mbar_init(b_full + s, 1); mbar_init(empty + s, 8); }   // empty: one arrival per consumer warp
         mbar_fence_init();
     }
-    if (warp == 1) {                                                       // TMEM: all 512 columns, one CTA per SM
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(tmem_slot)), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
-        // ===== TMA producer: activation tile [NT x 64] of K block kb =====
-        if (lane == 0) {
-            for (int kb = 0; kb < KB; kb++) {
-                const int s = kb % SB;
-                if (kb >= SB) mbar_wait(b_empty + s, (uint32_t) ((kb / SB - 1) & 1));
-                mbar_expect_tx(b_full + s, (uint32_t) b_stage);
-                tma_load_2d(sB + (size_t) s * b_stage, &xmap, (kb0 + kb) * BK, 0, b_full + s);
-                if (a.NT > 256) tma_load_2d(sB + (size_t) s * b_stage + a.box_rows * 128, &xmap, (kb0 + kb) * BK, 256, b_full + s);
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        if (lane == 0) {
-            const int n0 = a.NT > 256 ? 256 : a.NT, n1 = a.NT > 256 ? a.NT - 256 : 0;
-            const uint32_t id0 = instr_desc_f16(n0), id1 = instr_desc_f16(n1 > 0 ? n1 : 16);
-            for (int kb = 0; kb < KB; kb++) {
-                const int sa = kb % SA, sb = kb % SB;
-                mbar_wait(a_full + sa, (uint32_t) ((kb / SA) & 1));
-                mbar_wait(b_full + sb, (uint32_t) ((kb / SB) & 1));
-                tc_fence_after();
-                const uint32_t a_addr = smem_u32(sA + (size_t) sa * A_STAGE), b_addr = smem_u32(sB + (size_t) sb * b_stage);
-#pragma unroll
-                for (int k = 0; k < BK / 16; k++) {
-                    const uint64_t da = umma_desc(a_addr + k * 32);
-                    tc_mma_f16(tmem_base, da, umma_desc(b_addr + k * 32), id0, (kb | k) != 0);
-                    if (n1 > 0) tc_mma_f16(tmem_base + 256, da, umma_desc(b_addr + a.box_rows * 128 + k * 32), id1, (kb | k) != 0);
-                }
-                tc_commit(a_empty + sa);                                   // stages are free once these MMAs have read them
-                tc_commit(b_empty + sb);
-            }
-            tc_commit(acc_full);
-        }
-    } else {
-        // ===== dequant producers (2 threads per weight row) =====
-        const int t = threadIdx.x - 64, r = t >> 2, h = t & 3;
+    if (warp < 4) {
+        // ===== dequant producers (one thread per weight row) + the TMA of the activation tile =====
+        const int r = threadIdx.x;
         const size_t row = (size_t) min(m0 + r, a.W.M - 1);                // rows past M are computed from row M-1 and never stored
         using P = Prod<TYPE>;
-        typename P::Raw raw, raw1;                                         // the bytes of K blocks kb and kb + 1: two loads in flight per thread
-        typename P::Ptr pq;
+        typename P::Raw raw[4], raw1[4];                                   // the bytes of K blocks kb and kb + 1: two loads in flight per chunk pair
+        typename P::Ptr pq[4];
         if constexpr (P::FAST) {
-            const typename P::Ptr p0 = P::ptr(a.W, row, kb0, h);
-            pq = P::ptr(a.W, row, kb0 + (KB > 1 ? 1 : 0), h);
-            raw = P::load(p0, kb0, h); raw1 = P::load(pq, kb0 + (KB > 1 ? 1 : 0), h);
+#pragma unroll
+            for (int h = 0; h < 4; h++) {
+                const typename P::Ptr p0 = P::ptr(a.W, row, kb0, h);
+                pq[h] = P::ptr(a.W, row, kb0 + (KB > 1 ? 1 : 0), h);
+                raw[h] = P::load(p0, kb0, h); raw1[h] = P::load(pq[h], kb0 + (KB > 1 ? 1 : 0), h);
+            }
         }
         const int sw = r & 7;
-        const uint32_t st0 = smem_u32(sA) + (uint32_t) (r * 128 + ((h ^ sw) << 4)), st1 = smem_u32(sA) + (uint32_t) (r * 128 + (((4 + h) ^ sw) << 4));
+        const uint32_t st_row = smem_u32(sA) + (uint32_t) (r * 128);
         for (int kb = 0; kb < KB; kb++) {
-            const int s = kb % SA;
-            Chunks ch;
-            if constexpr (P::FAST) {
-                ch = P::deq(raw, kb0 + kb, h);
-                raw = raw1;
-                P::next(pq);                                                // -> K block kb0 + kb + 2
-                if (kb + 2 < KB) raw1 = P::load(pq, kb0 + kb + 2, h);       // two blocks ahead: an L2 / HBM round trip is longer than one block's MMA time
-            } else ch = dequant_generic(a.W, row, (kb0 + kb) * BK, h);
-            if (kb >= SA) mbar_wait(a_empty + s, (uint32_t) ((kb / SA - 1) & 1));
-            asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" :: "r"(st0 + (uint32_t) s * A_STAGE), "r"(ch.c[0].x), "r"(ch.c[0].y), "r"(ch.c[0].z), "r"(ch.c[0].w) : "memory");   // elements 8h .. 8h+7
-            asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" :: "r"(st1 + (uint32_t) s * A_STAGE), "r"(ch.c[1].x), "r"(ch.c[1].y), "r"(ch.c[1].z), "r"(ch.c[1].w) : "memory");   // elements 32+8h .. 32+8h+7
+            const int s = kb % ST;
+            if (kb >= ST) mbar_wait(empty + s, (uint32_t) ((kb / ST - 1) & 1));
+            if (r == 0) {
+                mbar_expect_tx(b_full + s, (uint32_t) B_STAGE);            // rows past N are zero-filled by TMA and still counted
+                tma_load_2d(sB + (size_t) s * B_STAGE, &xmap, (kb0 + kb) * BK, n0, b_full + s);
+            }
+#pragma unroll
+            for (int h = 0; h < 4; h++) {
+                Chunks ch;
+                if constexpr (P::FAST) {
+                    ch = P::deq(raw[h], kb0 + kb, h);
+                    raw[h] = raw1[h];
+                    P::next(pq[h]);                                        // -> K block kb0 + kb + 2
+                    if (kb + 2 < KB) raw1[h] = P::load(pq[h], kb0 + kb + 2, h);
+                } else ch = dequant_generic(a.W, row, (kb0 + kb) * BK, h);
+                const uint32_t st = st_row + (uint32_t) s * A_STAGE;
+                asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" :: "r"(st + (uint32_t) ((h ^ sw) << 4)), "r"(ch.c[0].x), "r"(ch.c[0].y), "r"(ch.c[0].z), "r"(ch.c[0].w) : "memory");         // elements 8h .. 8h+7
+                asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" :: "r"(st + (uint32_t) (((4 + h) ^ sw) << 4)), "r"(ch.c[1].x), "r"(ch.c[1].y), "r"(ch.c[1].z), "r"(ch.c[1].w) : "memory");   // elements 32+8h .. 32+8h+7
+            }
             fence_proxy_async();                                           // generic-proxy stores -> visible to the tensor core (async proxy)
             mbar_arrive(a_full + s);
         }
-        // ===== epilogue: TMEM -> registers -> global =====
-        mbar_wait(acc_full, 0);
-        tc_fence_after();
-        const int q = warp & 3;                                            // TMEM lane quarter this warp may access
-        const int half_id = (warp - 2) >> 2;                               // four warps share a quarter: 32-column chunks c = id, id + 4, ...
-        const int m = m0 + q * 32 + lane;
-        const int nchunks = (a.NT + 31) / 32;
-        for (int c = half_id; c < nchunks; c += PRODUCER_THREADS / 128) {
-            uint32_t v[32];
-            tmem_ld32(tmem_base + ((uint32_t) (q * 32) << 16) + (uint32_t) (c * 32), v);
-            if (m < a.W.M) {
-#pragma unroll
-                for (int j = 0; j < 32; j++) {
-                    const int n = c * 32 + j;
-                    if (n < a.N) {
-                        float y = __uint_as_float(v[j]);
-                        if (a.epi_gelu) { const float f = __half2float(__float2half_rn(y));
-                            y = __half2float(__float2half_rn(0.5f * f * (1.0f + tanhf(0.79788456080286535587989211986876f * f * (1.0f + 0.044715f * f * f))))); }
-                        if (a.ksplit > 1) atomicAdd(a.Y + (size_t) n * a.y_stride + m, y);
-                        else a.Y[(size_t) n * a.y_stride + m] = y;         // a warp writes 32 consecutive m: 128 B per store
-                    }
-                }
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "r"(512) : "memory");
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// 256 < N <= 512: CTA PAIR (cta_group::2).  ncu on the single-CTA kernel (profiles/r2_gemm_tc.md): the dequantisation producers wait for
-// free stages, yet the tensor pipe is only 66 % busy -- every CTA pulls its own copy of the 64 KB activation tile per K block, 64 B/clk
-// per SM against a chip-wide L2 throughput of ~6300 B/clk = 42.6 B/clk per SM: 42.6 / 64 = 0.665.  In a pair the B operand of one
-// tcgen05.mma.cta_group::2 (M = 256: the two CTAs' 128 weight rows, N = 256 tokens) is split between the two CTAs' shared memories and
-// read by both tensor cores, so each CTA loads only HALF of every activation tile (32 KB per K block, 32 B/clk).
-//   CTA r of the pair: weight rows [m0 + 128 r, +128) dequantised by its own producers (as before); tokens [128 r, 128 r + 128) of
-//   token tile 0 and [256 + h r, ...) of token tile 1 (h = half of that tile) loaded by its own TMA thread;
-//   the LEADER (rank 0) issues every MMA; a_full / b_full live in the leader (producers of the peer arrive remotely, the peer's TMA
-//   signals the leader's barrier through the cta_group::2 form), a_empty / b_empty / acc_full are multicast commits to both CTAs.
-__device__ __forceinline__ uint32_t cluster_rank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ uint32_t map_to_rank(uint32_t saddr, uint32_t rank) { uint32_t r; asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank)); return r; }
-// Arrival on a barrier of the peer CTA.  Default semantics (release at CTA scope), as CUTLASS signals the leader of a pair
-// (cutlass/arch/barrier.h: umma_arrive_2x1SM_sm0): what the arrival orders is this CTA's shared-memory tile -- made visible to the
-// async proxy by fence.proxy.async -- against the MMA the leader issues afterwards, and that MMA reads the tile through THIS CTA's
-// tensor core.  The .release.cluster / .acquire.cluster forms compile to MEMBAR.ALL.GPU + CCTL.IVALL per call (measured: 40 % slower).
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" :: "r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void cluster_barrier() { asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit_pair(uint64_t * bar) {          // arrives on `bar` in BOTH CTAs once the pair's MMAs issued so far are done
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" :: "r"(smem_u32(bar)), "h"((uint16_t) 3) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16_pair(uint32_t tmem_c, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, {%5, %5, %5, %5, %5, %5, %5, %5}, p;\n\t}"
-                 :: "r"(tmem_c), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(0) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_pair(void * smem_dst, const CUtensorMap * map, int c0, int c1, uint64_t * leader_bar) {
-    // executed by both CTAs; the peer bit of the barrier address is cleared so that the bytes are counted by the leader's barrier
-    asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                 :: "r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(leader_bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ uint32_t instr_desc_f16_m256(int n) { return (1u << 4) | ((uint32_t) (n >> 3) << 17) | ((uint32_t) (256 >> 4) << 24); }
-
-constexpr int SB2 = 4, B2_STAGE = 2 * 128 * 128;                           // per CTA and K block: two 128-token x 64-half boxes = 32 KB
-template <int TYPE>
-__global__ void __launch_bounds__(THREADS, 1) gemm_tc_pair_kernel(const __grid_constant__ CUtensorMap xmap, const GemmArgs a) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t * smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t) 1023);
-    uint8_t * sA = smem, * sB = smem + SA * A_STAGE;
-    uint64_t * bars = reinterpret_cast<uint64_t *>(sB + SB2 * B2_STAGE);
-    uint64_t * a_full = bars, * a_empty = bars + SA, * b_full = bars + 2 * SA, * b_empty = b_full + SB2, * acc_full = b_empty + SB2;
-    uint32_t * tmem_slot = reinterpret_cast<uint32_t *>(acc_full + 1);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_rank();
-    const int m0 = (int) blockIdx.x * BM;                                  // blockIdx.x = 2 * pair + rank: consecutive row tiles
-    const int KBT = a.W.K / BK;
-    const int kb0 = (int) ((int64_t) KBT * blockIdx.y / a.ksplit), KB = (int) ((int64_t) KBT * (blockIdx.y + 1) / a.ksplit) - kb0;
-    const int n1 = a.NT - 256, h1 = n1 / 2;                                // token tile 1 and its per-CTA half (n1 % 32 == 0)
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < SA; s++) { mbar_init(a_full + s, 2 * (PRODUCER_THREADS / 32)); mbar_init(a_empty + s, 1); }    // one arrival per producer warp of each CTA
-        for (int s = 0; s < SB2; s++) { mbar_init(b_full + s, 1); mbar_init(b_empty + s, 1); }
-        mbar_init(acc_full, 1);
-        mbar_fence_init();
-    }
-    cluster_barrier();                                                     // (both CTAs) before the paired TMEM allocation and any remote arrive
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(tmem_slot)), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_barrier();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        // ===== TMA: this CTA's halves of the two token tiles of K block kb =====
-        if (lane == 0) {
-            for (int kb = 0; kb < KB; kb++) {
-                const int s = kb % SB2;
-                if (kb >= SB2) mbar_wait(b_empty + s, (uint32_t) ((kb / SB2 - 1) & 1));
-                if (rank == 0) mbar_expect_tx(b_full + s, (uint32_t) (2 * B2_STAGE));      // both CTAs' bytes land on the leader's barrier
-                tma_load_2d_pair(sB + (size_t) s * B2_STAGE, &xmap, (kb0 + kb) * BK, (int) rank * 128, b_full + s);
-                tma_load_2d_pair(sB + (size_t) s * B2_STAGE + 128 * 128, &xmap, (kb0 + kb) * BK, 256 + (int) rank * h1, b_full + s);
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer: the leader CTA only =====
-        if (lane == 0 && rank == 0) {
-            const uint32_t id0 = instr_desc_f16_m256(256), id1 = instr_desc_f16_m256(n1);
-            for (int kb = 0; kb < KB; kb++) {
-                const int sa = kb % SA, sb = kb % SB2;
-                mbar_wait(a_full + sa, (uint32_t) ((kb / SA) & 1));
-                mbar_wait(b_full + sb, (uint32_t) ((kb / SB2) & 1));
-                tc_fence_after();
-                const uint32_t a_addr = smem_u32(sA + (size_t) sa * A_STAGE), b_addr = smem_u32(sB + (size_t) sb * B2_STAGE);
-#pragma unroll
-                for (int k = 0; k < BK / 16; k++) {
-                    const uint64_t da = umma_desc(a_addr + k * 32);
-                    tc_mma_f16_pair(tmem_base, da, umma_desc(b_addr + k * 32), id0, (kb | k) != 0);
-                    tc_mma_f16_pair(tmem_base + 256, da, umma_desc(b_addr + 128 * 128 + k * 32), id1, (kb | k) != 0);
-                }
-                tc_commit_pair(a_empty + sa);
-                tc_commit_pair(b_empty + sb);
-            }
-            tc_commit_pair(acc_full);
-        }
     } else {
-        // ===== dequant producers (4 threads per weight row), then the epilogue: exactly the single-CTA kernel's, except for the arrival =====
-        const int t = threadIdx.x - 64, r = t >> 2, h = t & 3;
-        const size_t row = (size_t) min(m0 + r, a.W.M - 1);
-        using P = Prod<TYPE>;
-        // the raw bytes of K blocks kb .. kb + PF - 1 are in flight per thread (a few registers each): with the activation traffic halved by
-        // the pair, what the MMAs wait for next is these loads (ncu: long-scoreboard stalls of the producers)
-        constexpr int PF = 4;
-        typename P::Raw raw[PF];
-        typename P::Ptr pq;
-        if constexpr (P::FAST) {
-            pq = P::ptr(a.W, row, kb0, h);
+        // ===== consumers: warpgroup g = 1, 2 owns weight rows [64 (g - 1), +64) of the tile =====
+        const int g = warp / 4 - 1, wq = warp & 3;
+        float acc[BN / 2];
 #pragma unroll
-            for (int i = 0; i < PF; i++) { if (i < KB) raw[i] = P::load(pq, kb0 + i, h); P::next(pq); }
+        for (int i = 0; i < BN / 2; i++) acc[i] = 0.f;
+        for (int kb = 0; kb < KB; kb++) {
+            const int s = kb % ST;
+            mbar_wait(a_full + s, (uint32_t) ((kb / ST) & 1));
+            mbar_wait(b_full + s, (uint32_t) ((kb / ST) & 1));
+            const uint32_t a_addr = smem_u32(sA + (size_t) s * A_STAGE) + g * 64 * 128, b_addr = smem_u32(sB + (size_t) s * B_STAGE);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < BK / 16; k++) Wgmma<BN>::mma(acc, wgmma_desc(a_addr + k * 32), wgmma_desc(b_addr + k * 32), 1);
+            wgmma_commit();
+            wgmma_wait<1>();                                               // the previous stage's MMAs are done: release it
+            if (kb > 0 && lane == 0) mbar_arrive(empty + (kb - 1) % ST);
         }
-        const int sw = r & 7;
-        const uint32_t st0 = smem_u32(sA) + (uint32_t) (r * 128 + ((h ^ sw) << 4)), st1 = smem_u32(sA) + (uint32_t) (r * 128 + (((4 + h) ^ sw) << 4));
-        const uint32_t full0 = map_to_rank(smem_u32(a_full), 0);          // the leader's a_full[0] as a shared::cluster address
-        for (int kbase = 0; kbase < KB; kbase += PF) {
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        // ===== epilogue: accumulator registers -> global =====
+        const int mr = m0 + g * 64 + wq * 16 + (lane >> 2);
 #pragma unroll
-            for (int u = 0; u < PF; u++) {
-                const int kb = kbase + u;
-                if (kb >= KB) break;
-                const int s = kb % SA;
-                Chunks ch;
-                if constexpr (P::FAST) {
-                    ch = P::deq(raw[u], kb0 + kb, h);
-                    if (kb + PF < KB) raw[u] = P::load(pq, kb0 + kb + PF, h);
-                    P::next(pq);
-                } else ch = dequant_generic(a.W, row, (kb0 + kb) * BK, h);
-                if (kb >= SA) mbar_wait(a_empty + s, (uint32_t) ((kb / SA - 1) & 1));
-                asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" :: "r"(st0 + (uint32_t) s * A_STAGE), "r"(ch.c[0].x), "r"(ch.c[0].y), "r"(ch.c[0].z), "r"(ch.c[0].w) : "memory");
-                asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" :: "r"(st1 + (uint32_t) s * A_STAGE), "r"(ch.c[1].x), "r"(ch.c[1].y), "r"(ch.c[1].z), "r"(ch.c[1].w) : "memory");
-                fence_proxy_async();                                           // generic-proxy stores -> visible to the tensor cores (async proxy)
-                __syncwarp();
-                if (lane == 0) { if (rank == 0) mbar_arrive(a_full + s); else mbar_arrive_cluster(full0 + (uint32_t) s * 8); }   // one arrival per warp on the LEADER's barrier
-            }
-        }
-        mbar_wait(acc_full, 0);
-        tc_fence_after();
-        const int q = warp & 3, half_id = (warp - 2) >> 2;
-        const int m = m0 + q * 32 + lane;
-        const int nchunks = (a.NT + 31) / 32;
-        for (int c = half_id; c < nchunks; c += PRODUCER_THREADS / 128) {
-            uint32_t v[32];
-            tmem_ld32(tmem_base + ((uint32_t) (q * 32) << 16) + (uint32_t) (c * 32), v);
-            if (m < a.W.M) {
+        for (int j = 0; j < BN / 8; j++) {
 #pragma unroll
-                for (int j = 0; j < 32; j++) {
-                    // accumulator column -> token: tile 0 = columns [0, 256), tile 1 = columns [256, 256 + n1)
-                    const int n = c * 32 + j;
-                    if (n < a.N) {
-                        float y = __uint_as_float(v[j]);
-                        if (a.epi_gelu) { const float f = __half2float(__float2half_rn(y));
-                            y = __half2float(__float2half_rn(0.5f * f * (1.0f + tanhf(0.79788456080286535587989211986876f * f * (1.0f + 0.044715f * f * f))))); }
-                        if (a.ksplit > 1) atomicAdd(a.Y + (size_t) n * a.y_stride + m, y);
-                        else a.Y[(size_t) n * a.y_stride + m] = y;
-                    }
+            for (int i = 0; i < 2; i++) {
+                const int m = mr + 8 * i;
+                if (m >= a.W.M) continue;
+#pragma unroll
+                for (int e = 0; e < 2; e++) {
+                    const int n = n0 + 8 * j + 2 * (lane & 3) + e;
+                    if (n >= a.N) continue;
+                    float y = acc[4 * j + 2 * i + e];
+                    if (a.epi_gelu) { const float f = __half2float(__float2half_rn(y));
+                        y = __half2float(__float2half_rn(0.5f * f * (1.0f + tanhf(0.79788456080286535587989211986876f * f * (1.0f + 0.044715f * f * f))))); }
+                    if (a.ksplit > 1) atomicAdd(a.Y + (size_t) n * a.y_stride + m, y);
+                    else a.Y[(size_t) n * a.y_stride + m] = y;
                 }
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    cluster_barrier();                                                     // the peer may still read this CTA's shared memory (B halves) / arrive on its barriers
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "r"(512) : "memory");
-}
-
-template <int TYPE>
-void launch_typed_pair(const CUtensorMap & map, const GemmArgs & a, cudaStream_t stream) {
-    const size_t smem = 1024 + (size_t) SA * A_STAGE + (size_t) SB2 * B2_STAGE + 256;
-    static bool set = false;
-    if (!set) { B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_pair_kernel<TYPE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); set = true; }
-    const int tiles = (a.W.M + BM - 1) / BM;
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned) ((tiles + 1) / 2 * 2), (unsigned) a.ksplit); cfg.blockDim = dim3(THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension; attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    B200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_tc_pair_kernel<TYPE>, map, a));
 }
 
 PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
@@ -546,12 +313,24 @@ PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
     return fn;
 }
 
-template <int TYPE>
-void launch_typed(const CUtensorMap & map, const GemmArgs & a, size_t smem, cudaStream_t stream) {
+template <int TYPE, int BN>
+void launch_typed(const CUtensorMap & map, const GemmArgs & a, cudaStream_t stream) {
+    const size_t smem = 1024 + (size_t) ST * (A_STAGE + BN * 128) + 256;
     static bool set = false;
-    if (!set) { B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<TYPE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); set = true; }
-    gemm_tc_kernel<TYPE><<<dim3((a.W.M + BM - 1) / BM, a.ksplit), THREADS, smem, stream>>>(map, a);
+    if (!set) { B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<TYPE, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem)); set = true; }
+    const dim3 grid((unsigned) ((a.N + BN - 1) / BN), (unsigned) ((a.W.M + BM - 1) / BM), (unsigned) a.ksplit);
+    gemm_tc_kernel<TYPE, BN><<<grid, THREADS, smem, stream>>>(map, a);
     B200_CUDA_CHECK(cudaGetLastError());
+}
+
+template <int BN>
+void launch_bn(const CUtensorMap & map, const GemmArgs & a, cudaStream_t stream) {
+    switch (a.W.type) {
+        case T_Q4_K: launch_typed<T_Q4_K, BN>(map, a, stream); break;
+        case T_Q4_0: launch_typed<T_Q4_0, BN>(map, a, stream); break;
+        case T_Q3_K: launch_typed<T_Q3_K, BN>(map, a, stream); break;
+        default:     launch_typed<-1, BN>(map, a, stream); break;           // generic element-wise dequantiser
+    }
 }
 
 } // namespace
@@ -560,37 +339,22 @@ void launch_typed(const CUtensorMap & map, const GemmArgs & a, size_t smem, cuda
 bool launch_gemm_tc(const WPlanes & W, const __half * X, int64_t x_stride, int N, float * Y, int64_t y_stride, int epi_gelu, cudaStream_t stream) {
     if (N > N_MAX || W.K % BK != 0 || (x_stride % 8) != 0 || ((uintptr_t) X & 15) != 0) return false;
     GemmArgs a;
-    a.W = W; a.Y = Y; a.y_stride = y_stride; a.N = N; a.NT = (N + 15) / 16 * 16; a.epi_gelu = epi_gelu;
-    a.box_rows = a.NT > 256 ? 256 : a.NT;
-    // fewer than ~100 row tiles cannot fill 148 SMs: split K in two (deterministic, see GemmArgs::ksplit)
-    const int tiles = (W.M + BM - 1) / BM;
+    a.W = W; a.Y = Y; a.y_stride = y_stride; a.N = N; a.epi_gelu = epi_gelu;
+    const int BN = N <= 64 ? 64 : N <= 128 ? 128 : 256;
+    // fewer than ~100 tiles cannot fill the 132 SMs of an H100: split K in two (deterministic, see GemmArgs::ksplit)
+    const int tiles = (W.M + BM - 1) / BM * ((N + BN - 1) / BN);
     a.ksplit = (tiles < 100 && !epi_gelu && W.K / BK >= 8 && !getenv("B200_GEMM_NOSPLIT")) ? 2 : 1;
     if (a.ksplit > 1) B200_CUDA_CHECK(cudaMemsetAsync(Y, 0, ((size_t) (N - 1) * y_stride + W.M) * sizeof(float), stream));
-    const bool pair = a.NT > 256 && (a.NT - 256) % 32 == 0 && !getenv("B200_GEMM_V1");      // CTA pair sharing the activation tile
     CUtensorMap map;
     const cuuint64_t gdim[2] = { (cuuint64_t) W.K, (cuuint64_t) N };
     const cuuint64_t gstr[1] = { (cuuint64_t) x_stride * 2 };
-    const cuuint32_t box[2] = { (cuuint32_t) BK, (cuuint32_t) (pair ? 128 : a.box_rows) };
+    const cuuint32_t box[2] = { (cuuint32_t) BK, (cuuint32_t) BN };
     const cuuint32_t estr[2] = { 1, 1 };
     const CUresult rc = get_encode()(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void *) X, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (rc != CUDA_SUCCESS) { fprintf(stderr, "b200: cuTensorMapEncodeTiled failed (%d)\n", (int) rc); exit(1); }
-    if (pair) {
-        switch (W.type) {
-            case T_Q4_K: launch_typed_pair<T_Q4_K>(map, a, stream); break;
-            case T_Q4_0: launch_typed_pair<T_Q4_0>(map, a, stream); break;
-            case T_Q3_K: launch_typed_pair<T_Q3_K>(map, a, stream); break;
-            default:     launch_typed_pair<-1>(map, a, stream); break;
-        }
-        return true;
-    }
-    const size_t b_stage = (size_t) a.box_rows * (a.NT > 256 ? 2 : 1) * 128;
-    const size_t smem = 1024 + (size_t) SA * A_STAGE + SB * b_stage + 256;
-    switch (W.type) {
-        case T_Q4_K: launch_typed<T_Q4_K>(map, a, smem, stream); break;
-        case T_Q4_0: launch_typed<T_Q4_0>(map, a, smem, stream); break;
-        case T_Q3_K: launch_typed<T_Q3_K>(map, a, smem, stream); break;
-        default:     launch_typed<-1>(map, a, smem, stream); break;        // generic element-wise dequantiser
-    }
+    if (BN == 64) launch_bn<64>(map, a, stream);
+    else if (BN == 128) launch_bn<128>(map, a, stream);
+    else launch_bn<256>(map, a, stream);
     return true;
 }

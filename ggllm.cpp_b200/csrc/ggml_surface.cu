@@ -1,5 +1,5 @@
 // ggml_surface.cu -- the reference's GPU operator surface (include/ggml_b200_cuda_surface.h == ggml-cuda.h:31-60)
-// implemented on the sm_100a kernels of this library.  Linking this instead of ggml-cuda.cu makes ggml.c's executor
+// implemented on the sm_90a kernels of this library.  Linking this instead of ggml-cuda.cu makes ggml.c's executor
 // (hook at ggml.c:15779-15790) and libfalcon.cpp's loader (libfalcon.cpp:1251) run unchanged.
 //
 // Residency model.  The reference decides per tensor: weights GPU / GPU_SPLIT (ggml_cuda_transform_tensor), graph

@@ -97,7 +97,7 @@ int    launch_attention(const float * qkv, const float * k_cache, const float * 
                         const AttnParams & p, float * scratch, cudaStream_t stream);
 size_t attention_scratch_bytes(const AttnParams & p);
 // N > 1 (prompt): tiled two-kernel version with a score scratch matrix (attention_prefill.cu)
-// attention_ws.cu: N > 8 on tcgen05, warp-specialised, over the fp16 shadow (p.k16 / p.vt16); false = not covered
+// attention_ws.cu: N > 8 on wgmma, warp-specialised, over the fp16 shadow (p.k16 / p.vt16); false = not covered
 bool   launch_attention_ws(const float * qkv, float * out, int64_t out_stride, const AttnParams & p, cudaStream_t stream);
 int    attention_ctx_pad(int n_ctx);
 size_t attention_shadow_halves(int n_head_kv, int n_ctx);           // halves per layer, for k16 and for vt16 each
@@ -106,7 +106,7 @@ size_t attention_prefill_scratch_bytes(int n_head, int n_tok, int T);
 void   launch_attention_prefill(const float * qkv, const float * k_cache, const float * v_cache, float * out, int64_t out_stride,
                                 const AttnParams & p, float * scratch, cudaStream_t stream);
 
-// ---- gemm.cu : Y[n][m] = sum_k W[m][k] * X[n][k], N large (prompt), tcgen05 tensor cores
+// ---- gemm.cu : Y[n][m] = sum_k W[m][k] * X[n][k], N large (prompt), wgmma tensor cores
 void   launch_mmq_gemm(const WPlanes & W, const __half * X, int64_t x_stride, int N, float * Y, int64_t y_stride,
                        int epi_gelu, void * workspace, size_t workspace_bytes, cudaStream_t stream);
 size_t mmq_gemm_workspace_bytes(const WPlanes & W, int N);

@@ -1,6 +1,6 @@
 // mmv_fast.cu -- the decode mat-vec for the types the BASELINE configs use (Q4_K, Q4_0), tuned for issue slots.
 //
-// ncu on the generic ring kernel (profiles/r1_mmv_q4k_ring.md) showed the mat-vec is NOT limited by HBM latency but
+// Profiling the generic ring kernel showed the mat-vec is NOT limited by HBM latency but
 // by instruction issue and the L1/shared-memory data path: 101 warp-instructions per 512 B of weights, most of them
 // address arithmetic, nibble shifts, 6-bit scale unpacking and shared-memory reads of the activation.  This kernel
 // removes them instead of hiding them:
@@ -132,8 +132,7 @@ __device__ __forceinline__ void mmv_body(const WPlanes & W, const FastX & X, flo
 
     // Programmatic dependent launch: the next kernel of the stream is released once this CTA is about to issue its last
     // weight loads.  Triggering earlier would park the dependent grid's CTAs at the head of the hardware queue for the
-    // whole duration of this kernel and keep the small attention kernels of the other stream from being scheduled
-    // (measured: profiles/r1_decode_timeline.md).
+    // whole duration of this kernel and keep the small attention kernels of the other stream from being scheduled.
     int gcount = 0;
     const int ekind = epi.kind; const float * r1p = epi.r1, * r2p = epi.r2;
     ring_run<TYPE, NT, J, D, false>(w, wp, row0, row1, wp, 0, 0, xr, aux, partial, gcount, 0, tid,
@@ -247,7 +246,7 @@ bool launch_mmv_fast_x(const WPlanes & W, const FastX & X, float * y, int64_t y_
         epi.qA = *e.qout; epi.qctr = e.qctr;
     }
     static int dist_bytes = -1;
-    // HBM -> L2 prefetch ahead of the ring: off by default, measured slower at every distance (profiles/r1_decode_timeline.md)
+    // HBM -> L2 prefetch ahead of the ring: off by default, measured slower at every distance
     if (dist_bytes < 0) { const char * s = getenv("B200_L2PF_KB"); dist_bytes = (s ? atoi(s) : 0) * 1024; }
     FastX Xp = X;
     Xp.l2_dist = W.stride[0] ? (int) (dist_bytes / W.stride[0]) : 0;
@@ -260,7 +259,7 @@ bool launch_mmv_fast_x(const WPlanes & W, const FastX & X, float * y, int64_t y_
 }
 // Which (type, K, activation mode) the fused single-stream decode path of engine.cu may rely on.  Q3_K has a fast mat-vec
 // (used through launch_mmv) but is NOT listed: its kernel is issue-bound, and the two-stream per-node path, which runs the
-// attention and MLP branches' mat-vecs concurrently, is faster for it (189 vs 180 tok/s, Falcon-40B).
+// attention and MLP branches' mat-vecs concurrently, is faster for it (Falcon-40B).
 bool mmv_fast_supports(int wtype, int K, int mode) {
     if (wtype != T_Q4_K && wtype != T_Q4_0) return false;
     const int P = wtype == T_Q4_K ? K / 32 : K / 32;

@@ -262,8 +262,7 @@ template <int G> __device__ __forceinline__ float transpose_reduce(const float (
 
 
 // HBM -> L2 prefetch of whole rows, `dist` rows ahead of the register ring.  The ring alone keeps 64 KB per SM in flight,
-// which at the ~2 us loaded HBM latency caps the stream at ~4.7 TB/s (ncu: 27 % of all stall samples sit on the first use
-// of a ring slot, profiles/r1_mmv_up_narrow.md); one bulk-prefetch instruction per plane and pass, issued by a single
+// which the loaded HBM latency turns into a cap on the stream (stalls sit on the first use of a ring slot); one bulk-prefetch instruction per plane and pass, issued by a single
 // thread, moves the latency the ring has to cover from HBM to L2.
 struct L2PF { const uint8_t * p[3]; uint32_t s[3]; int dist; };
 __device__ __forceinline__ void l2_prefetch_rows(const L2PF & pf, int a, int b) {       // rows [a, b) of every plane

@@ -186,7 +186,7 @@ __global__ void __launch_bounds__(LNR_THREADS) layernorm_q_reg_kernel(float * __
 // Decode (one row): the same LayerNorm + quantisation spread over a thread-block CLUSTER of ceil(n / 1024) <= 8 CTAs x 128 threads,
 // 8 values per thread.  The 1024-thread single-CTA kernel above needs a whole SM's registers, so it cannot become resident
 // before the previous mat-vec has drained, and its ~64 registers per thread leave no room to have gamma / beta in flight
-// early: 7 us between the end of wo and the first qkv row (profiles/r1_decode_timeline.md).  Here every CTA is small enough
+// early: a gap between the end of wo and the first qkv row.  Here every CTA is small enough
 // to sit beside the mat-vec's CTAs, loads its gamma / beta BEFORE griddepcontrol.wait, and after the wait pays one L2 round
 // trip plus two cluster reductions through distributed shared memory (fixed summation order: deterministic).
 #define LNC_THREADS 128
@@ -352,7 +352,7 @@ __global__ void scale_kernel(const float * __restrict__ a, float s, float * __re
 __global__ void f32_to_f16_kernel(const float * __restrict__ x, __half * __restrict__ y, int64_t n) {       // ggml_fp32_to_fp16_row
     for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x * blockDim.x) y[i] = __float2half_rn(x[i]);
 }
-static unsigned ew_grid(int64_t n) { int64_t g = (n + 255) / 256; return (unsigned) (g < 1 ? 1 : (g > 148 * 16 ? 148 * 16 : g)); }
+static unsigned ew_grid(int64_t n) { int64_t g = (n + 255) / 256; return (unsigned) (g < 1 ? 1 : (g > 132 * 16 ? 132 * 16 : g)); }
 void launch_f32_to_f16(const float * x, __half * y, int64_t n, cudaStream_t s) { f32_to_f16_kernel<<<ew_grid(n), 256, 0, s>>>(x, y, n); B200_CUDA_CHECK(cudaGetLastError()); }
 void launch_gelu(const float * x, float * y, int64_t n, cudaStream_t s) { gelu_kernel<<<ew_grid(n), 256, 0, s>>>(x, y, n); B200_CUDA_CHECK(cudaGetLastError()); }
 void launch_add(const float * a, const float * b, float * y, int64_t n, cudaStream_t s) { add_kernel<<<ew_grid(n), 256, 0, s>>>(a, b, y, n); B200_CUDA_CHECK(cudaGetLastError()); }
@@ -416,8 +416,8 @@ __global__ void rope_kv_append_kernel(float * __restrict__ qkv, float * __restri
     trace_end(p.trace);
 }
 // The same work for a batch of tokens (prompt).  The single-token kernel above recomputes the 32 rotation angles of a position in every
-// one of its (n_head + 2 n_head_kv) x n_tok tiny CTAs and scatters V^T two bytes at a time (78 us per Falcon-40B layer at 512 tokens,
-// as long as the attention itself).  Here one CTA per token computes its cos / sin once and walks the row coalesced, and the V^T shadow
+// one of its (n_head + 2 n_head_kv) x n_tok tiny CTAs and scatters V^T two bytes at a time (at 512 tokens
+// about as long as the attention itself).  Here one CTA per token computes its cos / sin once and walks the row coalesced, and the V^T shadow
 // is written by extra CTAs that transpose 64 tokens x 64 dims through shared memory (128-byte rows).  Same arithmetic, same bits.
 __global__ void __launch_bounds__(256) rope_kv_append_batch_kernel(float * __restrict__ qkv, float * __restrict__ kc, float * __restrict__ vc, AttnParams p, float theta_scale) {
     const int D = p.head_dim, half = D / 2, H = p.n_head, HKV = p.n_head_kv, N = p.n_tok;

@@ -149,7 +149,7 @@ void wplanes_alloc_random(WPlanes & W, int type, int K, int M, uint64_t seed, cu
     uint8_t * base = nullptr;
     B200_CUDA_CHECK(cudaMalloc(&base, W.bytes));
     for (int i = 0; i < ts.n_planes; i++) W.p[i] = base + reinterpret_cast<size_t>(W.p[i]);
-    fill_random_kernel<<<148 * 8, 256, 0, stream>>>(W, ts, seed);
+    fill_random_kernel<<<132 * 8, 256, 0, stream>>>(W, ts, seed);
     B200_CUDA_CHECK(cudaGetLastError());
 }
 

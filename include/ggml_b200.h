@@ -1,5 +1,5 @@
 /*
- * ggml_b200.h -- C ABI of libggml_b200.so, the B200 (sm_100a) quantized-inference backend for ggllm.cpp.
+ * ggml_b200.h -- C ABI of libggml_b200.so, the H100 (sm_90a) quantized-inference backend for ggllm.cpp.
  *
  * Plain C: pointers, sizes and ggml type ids (enum ggml_type, ggml.h:241-262) only.  No torch / C++ types.
  * Pointers named *_dev are CUDA device pointers on the current device; everything else is host memory.
@@ -78,7 +78,7 @@ void        b200_actq_download(const b200_actq * a, int8_t * q, float * d, float
 /* ---- y[n][m] = sum_k W[m][k] x[n][k].  Replaces ggml_cuda_mul_mat (ggml-cuda.cu:2931-2951):
  * N == 1..b200_mmv_max_n(): fused dequantise + integer-dot mat-vec (replaces dequantize_mul_mat_vec*,
  *                            ggml-cuda.cu:475-845, 1121-1171)
- * larger N               : tcgen05 tensor-core GEMM with fused dequantisation (replaces to_fp16_cuda +
+ * larger N               : wgmma tensor-core GEMM with fused dequantisation (replaces to_fp16_cuda +
  *                            float_to_half + cublasGemmEx, ggml-cuda.cu:2353-2403)
  * x/y are fp32 device buffers with row strides in floats. */
 void   b200_mul_mat(const b200_weight * w, const float * x_dev, int64_t x_stride, int N, float * y_dev, int64_t y_stride);
@@ -103,7 +103,7 @@ int    b200_mul_mat_vec_q_chain(const b200_weight * w, const b200_actq * a_in, f
 int    b200_quantize_weights(int ggml_type, const float * x_dev, void * blocks_dev, int64_t n_elems);
 int    b200_mmv_max_n(void);
 /* the GEMM half alone, on fp16 activations x[n][k] already on the device (what b200_mul_mat does after quantising):
- * impl 1 = tcgen05 tensor-core kernel (returns 0 if the shape is not covered: N > 512 or K % 64 != 0),
+ * impl 1 = wgmma tensor-core kernel (returns 0 if the shape is not covered: N > 512 or K % 64 != 0),
  * impl 0 = CUDA-core kernel with identical operand rounding (the test reference for impl 1). */
 int    b200_mul_mat_f16(const b200_weight * w, const void * x_f16_dev, int64_t x_stride, int N, float * y_dev, int64_t y_stride,
                         int epilogue_gelu, int impl);

@@ -1,4 +1,4 @@
-"""CPU tests: the C-ABI library builds for sm_100a, loads without a GPU and exports every symbol include/*.h declares."""
+"""CPU tests: the C-ABI library builds for sm_90a, loads without a GPU and exports every symbol include/*.h declares."""
 import ctypes
 import os
 import re
@@ -53,16 +53,16 @@ def test_no_gpu_means_loud_failure_not_fallback(lib):
         b.init(0)
 
 
-def test_sass_is_sm100a_with_tma(lib):
-    """the shipped cubin targets sm_100a only and the mat-vec stages activations with a bulk (TMA) copy"""
+def test_sass_is_sm90a_with_tma(lib):
+    """the shipped cubin targets sm_90a only and the mat-vec stages activations with a bulk (TMA) copy"""
     import subprocess
     import ggllm_cpp_b200.binding as b
     out = subprocess.run(["cuobjdump", "-lelf", b.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out and "sm_90" not in out and "sm_80" not in out
-    # one disassembly pass: the mat-vec stages activations with a TMA bulk copy; the tensor-core paths are really in the binary: tcgen05.mma
-    # (prompt GEMM / attention), TMA tensor loads, tcgen05.ld, and the warp-level mma.sync + cp.async rings of the long-context decode attention
+    assert "sm_90a" in out and "sm_100" not in out and "sm_80" not in out
+    # one disassembly pass: the mat-vec stages activations with a TMA bulk copy; the tensor-core paths are really in the binary: wgmma
+    # (prompt GEMM / attention), TMA tensor loads, and the warp-level mma.sync + cp.async rings of the long-context decode attention
     p = subprocess.Popen(["cuobjdump", "-sass", b.LIB_PATH], stdout=subprocess.PIPE, text=True)
-    counts = dict.fromkeys(("UBLKCP", "UTCHMMA", "UTMALDG", "LDTM", "HMMA", "LDGSTS", "IDP.4A"), 0)
+    counts = dict.fromkeys(("UBLKCP", "HGMMA", "UTMALDG", "HMMA", "LDGSTS", "IDP.4A"), 0)
     for line in p.stdout:
         for op in counts:
             if op in line:

@@ -12,7 +12,7 @@ pytestmark = pytest.mark.gpu
 HOOK = os.path.join(po.HERE, "_ref", "libfalcon_hook.so")
 
 
-@pytest.mark.skipif(not os.path.exists(HOOK), reason="oracle/_ref/libfalcon_hook.so not present (built where /root/reference exists)")
+@pytest.mark.skipif(not os.path.exists(HOOK), reason="oracle/_ref/libfalcon_hook.so not present (built by make -C oracle ref from the reference sources)")
 @pytest.mark.parametrize("takeover", [True, False])
 @pytest.mark.parametrize("hp,wt,ftype,overrides", [(TINY_40B, po.Q4_K, 15, None), (TINY_7B, po.Q4_0, 2, None),
                                                    (TINY_40B, po.Q4_K, 15, {"lm_head": po.F16})])      # a --leave-output-tensor file
@@ -41,7 +41,7 @@ def test_reference_eval_runs_on_our_operator_surface(gpu, tmp_path, hp, wt, ftyp
         assert np.abs(g - w).max() <= 2e-2 * S and np.median(np.abs(g - w)) <= 2e-3 * S
         tight.append(bool(np.median(np.abs(g - w)) <= 2e-5 * S))
     assert sum(tight) * 2 >= len(tight), tight
-    # (2) 12 tokens: the N > 8 (tcgen05 GEMM, fp16 operands) branch of the hook, then decode over the KV cache it wrote.
+    # (2) 12 tokens: the N > 8 (wgmma GEMM, fp16 operands) branch of the hook, then decode over the KV cache it wrote.
     #     Tolerance: the GEMM-path bound (max 3e-2 * S, median 5e-3 * S)
     prompt = np.array([11] + list(range(100, 111)), np.int32)
     got, want = ref.eval(prompt, 0, n_threads=2), o.eval(prompt, 0, all_logits=True)

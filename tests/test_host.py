@@ -184,7 +184,7 @@ def test_fp16_split_products_reach_fp32_dot_accuracy():
 
 
 def test_launch_list_tool_pivots_an_ncu_csv(tmp_path):
-    """tools/launch_list.py (the script behind profiles/r2_bench_launches.csv and r2_traffic.json): one row per launch, the last COMPLETE
+    """tools/launch_list.py (pivots an Nsight Compute launch list): one row per launch, the last COMPLETE
     decode step only, DRAM bytes per mat-vec launch"""
     import subprocess, csv as _csv, json
     ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -240,10 +240,10 @@ def test_attention(gpu, orc, n_head, n_head_kv, n_tok, n_past):
 
 @pytest.mark.parametrize("t,M,K,N,gelu", [(po.Q4_K, 256, 512, 40, 0), (po.Q4_K, 1000, 1024, 300, 0), (po.Q4_K, 384, 2048, 512, 1),
                                           (po.Q4_0, 200, 256, 17, 0), (po.Q6_K, 128, 512, 64, 0), (po.Q4_K, 128, 8192, 9, 0), (po.Q4_K, 640, 1024, 512, 0),
-                                          (po.Q6_K, 300, 512, 260, 0), (po.Q4_K, 520, 2048, 400, 1),       # N > 256: the CTA-pair kernel
+                                          (po.Q6_K, 300, 512, 260, 0), (po.Q4_K, 520, 2048, 400, 1),       # N > 256: two token tiles
                                           (po.Q4_0, 300, 4544, 512, 0), (po.Q3_K, 520, 2048, 400, 0), (po.Q3_K, 130, 1024, 77, 1), (po.Q4_0, 71, 576, 130, 0)])
 def test_tensor_core_gemm_matches_cuda_core_gemm(gpu, orc, t, M, K, N, gelu):
-    """tcgen05 kernel vs the CUDA-core kernel on identical fp16 operands: only the fp32 accumulation order differs.
+    """wgmma kernel vs the CUDA-core kernel on identical fp16 operands: only the fp32 accumulation order differs.
     Then both against the exact fp64 product of the fp16-rounded operands."""
     rng = np.random.default_rng(M + K + N)
     wq = _weights(orc, t, M, K, seed=3)
@@ -269,7 +269,7 @@ def test_tensor_core_gemm_matches_cuda_core_gemm(gpu, orc, t, M, K, N, gelu):
 def test_tensor_core_gemm_operand_is_the_exact_fp16_weight(gpu, orc, t, N):
     """One-hot activation rows read the dequantised A operand back through the tensor cores: Y[n][m] = fp16(w[m][k_n]) exactly.
     Pins the per-type dequantisation producers of gemm_tc.cu (Q4_K fp32 fma; Q4_0 / Q3_K half arithmetic; generic for the rest),
-    in the single-CTA kernel (N = 200) and the CTA-pair kernel (N = 512), to dequantize_row_* + one fp16 rounding."""
+    with one token tile (N = 200) and two (N = 512), to dequantize_row_* + one fp16 rounding."""
     M, K = 300, 1024
     wq = _weights(orc, t, M, K, seed=11)
     W = gpu.Weight(t, K, M, wq)
@@ -374,7 +374,7 @@ def test_full_size_matvec_all_rows(gpu, orc, t, K, M):
 
 @pytest.mark.parametrize("K,M,N", [(8192, 32768, 512), (32768, 8192, 512), (8192, 9216, 384)])
 def test_full_size_gemm_tensor_core_vs_cuda_core(gpu, K, M, N):
-    """BASELINE config 3 shapes (Falcon-40B ffn_up / ffn_down / qkv at n_batch 512): the tcgen05 kernel and the CUDA-core
+    """BASELINE config 3 shapes (Falcon-40B ffn_up / ffn_down / qkv at n_batch 512): the wgmma kernel and the CUDA-core
     reference kernel read the same Q4_K blocks and the same fp16 activations; only the fp32 accumulation order differs."""
     import ggllm_cpp_b200.ggcc as ggcc
     rng = np.random.default_rng(K + M + N)
@@ -388,7 +388,7 @@ def test_full_size_gemm_tensor_core_vs_cuda_core(gpu, K, M, N):
     a, b = y0.download(np.float32, (N, M)), y1.download(np.float32, (N, M))
     scale = float(np.abs(a).max())
     assert np.isfinite(b).all() and scale > 0
-    # fp32 reassociation over K products (and the two-way K split of the tcgen05 kernel): grows like sqrt(K)
+    # fp32 reassociation over K products (and the two-way K split of the wgmma kernel): grows like sqrt(K)
     grow = (K / 8192.0) ** 0.5
     assert np.abs(a - b).max() <= 1e-4 * grow * scale, (float(np.abs(a - b).max()), scale)
     assert np.median(np.abs(a - b)) <= 5e-6 * grow * scale, (float(np.median(np.abs(a - b))), scale)

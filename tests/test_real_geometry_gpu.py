@@ -4,7 +4,7 @@ Falcon-7B 4544/71/1, Falcon-180B 14848/232/8), not only at the tiny test shapes:
   * the 8-CTA thread-block-cluster LayerNorm (n_embd 8192), its 5-CTA ragged form (4544) and the two-pass register kernel (14848)
   * split-KV decode attention with G = 16 / 71 / 29 query heads per KV head, with and without the Q8 hand-over to `wo`,
     at n_past 0 / 300 / 2040 / 8184 of an 8192-token context
-  * the tcgen05 prompt attention over 16 key tiles (T = 2048) and the tcgen05 GEMM at the real K
+  * the wgmma prompt attention over 16 key tiles (T = 2048) and the wgmma GEMM at the real K
   * whole evals (2 layers, vocabulary 2048) through b200_falcon_eval at those positions
 
 The 2-layer models carry well-formed pseudo-random blocks (ggcc.random_blocks: what bench.py's synthetic models hold) and the
@@ -92,7 +92,7 @@ def test_decode_at_real_geometry(gpu, geom, wtype):
 
 
 def test_prompt_chunk_at_real_geometry(gpu):
-    """a 96-token chunk ending at position 2048 of the Falcon-40B geometry: tcgen05 GEMMs at K = 8192 / 32768 and tcgen05 attention over
+    """a 96-token chunk ending at position 2048 of the Falcon-40B geometry: wgmma GEMMs at K = 8192 / 32768 and wgmma attention over
     16 key tiles (T = 2048), against the oracle.  Tolerance: the GEMM-path bound of tests/test_falcon_gpu.py (fp16 operands)."""
     f, o = model_pair(gpu, "40b", po.Q4_K, n_batch=96)
     toks = (np.arange(96, dtype=np.int32) * 7 + 13) % 2048
@@ -196,7 +196,7 @@ def test_attention_decode_node(gpu, orc, n_head, n_head_kv, wtype, n_past):
 
 @pytest.mark.parametrize("n_head,n_head_kv,n_tok,n_past", [(128, 8, 512, 1536), (128, 8, 200, 700), (71, 1, 130, 1918), (232, 8, 64, 4032)])
 def test_prompt_attention_many_key_tiles(gpu, orc, n_head, n_head_kv, n_tok, n_past):
-    """tcgen05 prompt attention with up to 32 key tiles of 128 (BASELINE config 3 runs 512-token chunks up to T = 2048) against the
+    """wgmma prompt attention with up to 32 key tiles of 128 (BASELINE config 3 runs 512-token chunks up to T = 2048) against the
     numpy / oracle restatement.  Tolerance: Q, K, V are rounded to fp16 (2^-11 relative) -> atol 5e-3, median 5e-4 on O(1) outputs."""
     rng = np.random.default_rng(n_tok + n_past)
     hd, n_ctx = 64, n_past + n_tok
@@ -216,7 +216,7 @@ def test_prompt_attention_many_key_tiles(gpu, orc, n_head, n_head_kv, n_tok, n_p
 
 @pytest.mark.parametrize("t,K,M,N", [(po.Q4_K, 8192, 256, 512), (po.Q4_K, 32768, 128, 512), (po.Q4_0, 4544, 192, 300), (po.Q3_K, 8192, 128, 256)])
 def test_full_k_gemm_against_oracle_columns(gpu, orc, t, K, M, N):
-    """b200_mul_mat (N > 8: quantise -> fp16 -> tcgen05 GEMM with fused dequantisation) at the real contraction lengths against the
+    """b200_mul_mat (N > 8: quantise -> fp16 -> wgmma GEMM with fused dequantisation) at the real contraction lengths against the
     ORACLE's mul_mat (not against our own CUDA-core kernel): |diff| <= 2e-3 * sum_k |w_k x_k| per output (fp16 rounding of both operands,
     2^-11 each, random signs) and a tight median."""
     rng = np.random.default_rng(K + M)

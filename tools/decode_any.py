@@ -1,10 +1,11 @@
-"""Decode tok/s of a random-init Falcon model of a given shape / weight type (run on the GPU box).
+"""Decode tok/s of a random-init Falcon model of a given shape / weight type (needs an H100).
 usage: python tools/decode_any.py 7b|40b <ggml type id> [steps]"""
 import sys, os, json
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import ggllm_cpp_b200.binding as b
 import ggllm_cpp_b200.ggcc as ggcc
+from bench import peaks
 
 SHAPES = {"7b": dict(n_vocab=65024, n_embd=4544, n_head=71, n_head_kv=1, n_layer=32, falcon_type=7),
           "40b": dict(n_vocab=65024, n_embd=8192, n_head=128, n_head_kv=8, n_layer=60, falcon_type=40),
@@ -25,4 +26,4 @@ L.b200_event_record(e1, f.stream()); L.b200_event_synchronize(e1)
 ms = L.b200_event_elapsed_ms(e0, e1) / steps
 wb = f.weight_bytes()
 print(json.dumps(dict(model=sys.argv[1], type=t, n_past=start, ms_per_tok=round(ms, 4), tok_s=round(1e3 / ms, 1), weight_GB=round(wb / 1e9, 3),
-                      roofline_tok_s=round(6586.1e9 / wb, 1), frac=round(wb / (ms / 1e3) / 6586.1e9, 3), launches=f.last_launches())))
+                      roofline_tok_s=round(peaks()[0] * 1e9 / wb, 1), frac=round(wb / (ms / 1e3) / (peaks()[0] * 1e9), 3), launches=f.last_launches())))

@@ -1,8 +1,9 @@
-"""Micro-benchmark of the prompt GEMM (tcgen05) on Falcon-40B shapes, N = 512 tokens (run on the GPU box)."""
+"""Micro-benchmark of the prompt GEMM (wgmma) on Falcon-40B shapes, N = 512 tokens (needs an H100)."""
 import sys, os, json
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import ggllm_cpp_b200.binding as b
+from bench import peaks
 
 def main():
     b.init(0)
@@ -25,7 +26,7 @@ def main():
         L.b200_event_record(e1, None); L.b200_event_synchronize(e1)
         ms = L.b200_event_elapsed_ms(e0, e1) / reps
         fl = 2.0 * K * M * N
-        print(json.dumps(dict(type=t, K=K, M=M, N=N, us=round(ms * 1e3, 1), TFLOPs=round(fl / ms / 1e9, 1), frac_of_1451=round(fl / ms / 1e9 / 1451.1, 3))), flush=True)
+        print(json.dumps(dict(type=t, K=K, M=M, N=N, us=round(ms * 1e3, 1), TFLOPs=round(fl / ms / 1e9, 1), frac_of_peak=round(fl / ms / 1e9 / peaks()[1], 3))), flush=True)
         W.free()
 
 if __name__ == "__main__":

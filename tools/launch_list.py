@@ -1,7 +1,7 @@
 """Pivot an ncu launch list (`ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum --clock-control none --csv
 --log-file raw.csv <command>`) into one row per launch, keep the LAST decode step (from the last embedding gather to the end), and print a
 per-kernel table.  With --traffic the DRAM bytes per mat-vec launch are written as json (bench.py reads it for roofline.traffic).
-usage: python tools/launch_list.py raw.csv out.csv [--traffic profiles/r2_traffic.json] [--all]"""
+usage: python tools/launch_list.py raw.csv out.csv [--traffic traffic.json] [--all]"""
 import csv, sys, json, collections, re
 
 def main():

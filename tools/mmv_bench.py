@@ -1,9 +1,10 @@
-"""Micro-benchmark of the decode mat-vec kernel on model shapes (run on the GPU box).
-Rotates through enough distinct weight matrices that every launch reads cold HBM (> 126 MB L2)."""
+"""Micro-benchmark of the decode mat-vec kernel on model shapes (needs an H100).
+Rotates through enough distinct weight matrices that every launch reads cold HBM (> 50 MB L2)."""
 import sys, os, json
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import ggllm_cpp_b200.binding as b
+from bench import peaks
 
 def main():
     b.init(0)
@@ -30,7 +31,7 @@ def main():
                 for w in Ws: L.b200_mul_mat_vec_q(w.h, A.h, yd.ptr, M, 0, None, None)
             L.b200_event_record(e1, None); L.b200_event_synchronize(e1)
             ms = L.b200_event_elapsed_ms(e0, e1) / (reps * nmat)
-            print(json.dumps(dict(type=t, K=K, M=M, us=round(ms * 1e3, 2), GBs=round(nbytes / ms / 1e6, 1), frac_of_6586=round(nbytes / ms / 1e6 / 6586.1, 3))), flush=True)
+            print(json.dumps(dict(type=t, K=K, M=M, us=round(ms * 1e3, 2), GBs=round(nbytes / ms / 1e6, 1), frac_of_peak=round(nbytes / ms / 1e6 / peaks()[0], 3))), flush=True)
             for w in Ws: w.free()
 
 if __name__ == "__main__":

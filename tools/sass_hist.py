@@ -1,11 +1,11 @@
 """SASS opcode histogram of every kernel in the built objects (runs on the CPU box: cuobjdump only).
-usage: python tools/sass_hist.py > profiles/r2_sass_histograms.md
-Evidence that the hot kernels are Blackwell-native: UTCHMMA (tcgen05.mma), UTMALDG (TMA tensor loads), LDTM (tcgen05.ld),
-UTCBAR (tcgen05.commit), UBLKCP (TMA bulk copy), IDP.4A (dp4a) and no F2I.U8.F16 (see profiles/r1_notes_for_next_round.md)."""
+usage: python tools/sass_hist.py > sass_histograms.md
+Evidence that the hot kernels are Hopper-native: HGMMA (wgmma), UTMALDG (TMA tensor loads), UBLKCP (TMA bulk copy), HMMA (mma.sync),
+LDGSTS (cp.async), IDP.4A (dp4a) and no F2I.U8.F16."""
 import collections, glob, os, re, subprocess, sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-KEY = ["UTCHMMA", "UTCBAR", "UTMALDG", "UBLKCP", "LDGSTS", "LDTM", "STTM", "IDP", "MUFU", "F2FP", "HMUL2", "HMMA", "SYNCS", "FENCE", "CCTL", "MEMBAR", "F2I"]
+KEY = ["HGMMA", "UTMALDG", "UBLKCP", "LDGSTS", "IDP", "MUFU", "F2FP", "HMUL2", "HMMA", "SYNCS", "FENCE", "CCTL", "MEMBAR", "F2I"]
 print("# SASS opcode histograms of the shipped kernels (cuobjdump -sass ggllm.cpp_b200/csrc/*.o)\n")
 print("Per kernel: total instructions, then the counts of the opcodes that identify the hardware path.\n")
 for obj in sorted(glob.glob(os.path.join(ROOT, "ggllm.cpp_b200", "csrc", "*.o"))):
