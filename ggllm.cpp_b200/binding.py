@@ -24,7 +24,7 @@ PART_B = ["b200_falcon_create", "b200_falcon_set_tensor", "b200_falcon_set_tenso
           "b200_ggcc_read_hparams", "b200_falcon_free", "b200_falcon_weight_bytes", "b200_nccl_unique_id",
           "b200_falcon_init_pipeline", "b200_falcon_eval", "b200_falcon_decode_dev", "b200_falcon_logits_dev", "b200_falcon_generate_greedy",
           "b200_falcon_last_launches", "b200_attention_long_launches", "b200_falcon_last_ms", "b200_falcon_stream", "b200_falcon_profile_matvec",
-          "b200_falcon_kv_read", "b200_falcon_kv_write", "b200_falcon_kv_fill_random", "b200_falcon_generate", "b200_falcon_load_seconds", "b200_falcon_save_kv", "b200_falcon_load_kv"]
+          "b200_falcon_kv_read", "b200_falcon_kv_write", "b200_falcon_kv_shadow_read", "b200_falcon_kv_fill_random", "b200_falcon_generate", "b200_falcon_load_seconds", "b200_falcon_save_kv", "b200_falcon_load_kv"]
 
 
 def build(verbose=False):
@@ -62,6 +62,7 @@ def lib():
             "b200_layernorm_q": (None, [vp, i64, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32]),
             "b200_attention_decode": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]),
             "b200_falcon_kv_read": (i32, [vp, i32, i32, i32, vp, vp]), "b200_falcon_kv_write": (i32, [vp, i32, i32, i32, vp, vp]),
+            "b200_falcon_kv_shadow_read": (i32, [vp, i32, i32, i32, vp, vp]),
             "b200_falcon_kv_fill_random": (i32, [vp, i32, i32, C.c_uint64]),
             "b200_sampler_create": (vp, [vp, vp, i32]), "b200_sampler_sample": (i32, [vp, vp, i32]), "b200_sampler_free": (None, [vp]),
             "b200_falcon_generate": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, vp]),
@@ -335,6 +336,14 @@ class Falcon:
         k, v = np.ascontiguousarray(k, np.float32), np.ascontiguousarray(v, np.float32)
         if self.L.b200_falcon_kv_write(self.h, layer, pos, k.shape[0], _np_ptr(k), _np_ptr(v)) != 0:
             raise RuntimeError("b200_falcon_kv_write: bad layer / range")
+
+    def kv_shadow_read(self, layer, pos, n):
+        """-> (k16 [n][n_head_kv][head_dim], vt16 [n_head_kv][head_dim][n]) of the fp16 cache copy, as uint16 bit patterns"""
+        hkv, hd = self.hp["n_head_kv"], self.hp["n_embd"] // self.hp["n_head"]
+        k, vt = np.empty((n, hkv, hd), np.uint16), np.empty((hkv, hd, n), np.uint16)
+        if self.L.b200_falcon_kv_shadow_read(self.h, layer, pos, n, _np_ptr(k), _np_ptr(vt)) != 0:
+            raise RuntimeError("b200_falcon_kv_shadow_read: no fp16 copy, bad layer or range")
+        return k, vt
 
     def save_kv(self, path, n_tokens):
         if self.L.b200_falcon_save_kv(self.h, path.encode(), n_tokens) != 0:

@@ -19,7 +19,9 @@
 // a K / V tile serves all of them) x all visible keys in tiles of 128; CTAs with the most key tiles are scheduled first.
 // Shared memory 97 KB.
 // Precision: Q, K, V rounded to fp16, fp32 accumulation, P exact; the row sum is an fp32 sum of the fp16 probabilities (the CPU's is
-// double).  Tolerance: tests/test_kernels_gpu.py::test_attention (atol 5e-3, median 5e-4), logits inside the GEMM-path bound.
+// double).  Keys >= T are never loaded (the tensor maps end at T), so stale cache rows cannot reach the P V product.
+// Tolerance: tests/test_attention_exact_gpu.py holds the kernel to an exact restatement of these roundings (tests/attn_exact.py)
+// within a per-element bound; logits inside the GEMM-path bound.
 #include "kernels.h"
 #include "wgmma.cuh"
 #include <cuda.h>
@@ -267,9 +269,12 @@ bool launch_attention_ws(const float * qkv, float * out, int64_t out_stride, con
     a.n_head_kv = p.n_head_kv; a.G = p.n_head / p.n_head_kv; a.n_tok = p.n_tok; a.n_past = p.n_past; a.T = p.n_past + p.n_tok;
     a.rows = a.G * p.n_tok; a.qkv_stride = p.qkv_stride; a.out_stride = out_stride;
     const int ctx_pad = attention_ctx_pad(p.n_ctx);
+    // Both maps end at key T, not at n_ctx / ctx_pad: TMA zero-fills the rest of the last key tile.  Cache rows >= T are stale (an earlier
+    // sequence, kv_write, load_kv) and may hold NaN or, for an fp32 value beyond 65504, Inf in the shadow; the masked probabilities are
+    // exact zeros, but 0 x NaN and 0 x Inf in the P V product are NaN.
     CUtensorMap kmap, vmap;
     {   // k16 [n_ctx][n_head_kv][64]: box = 128 keys x 1 head x 64 dims -> 128 rows of 128 B
-        const cuuint64_t gdim[3] = { 64, (cuuint64_t) p.n_head_kv, (cuuint64_t) p.n_ctx };
+        const cuuint64_t gdim[3] = { 64, (cuuint64_t) p.n_head_kv, (cuuint64_t) a.T };
         const cuuint64_t gstr[2] = { 128, (cuuint64_t) p.n_head_kv * 128 };
         const cuuint32_t box[3] = { 64, 1, 128 }, estr[3] = { 1, 1, 1 };
         const CUresult rc = get_encode()(&kmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void *) p.k16, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
@@ -277,7 +282,7 @@ bool launch_attention_ws(const float * qkv, float * out, int64_t out_stride, con
         if (rc != CUDA_SUCCESS) { fprintf(stderr, "b200: cuTensorMapEncodeTiled(k16) failed (%d)\n", (int) rc); exit(1); }
     }
     {   // vt16 [n_head_kv][64][ctx_pad]: box = 64 keys x 64 dims x 1 head -> 64 rows of 128 B (one half of a 128-key tile)
-        const cuuint64_t gdim[3] = { (cuuint64_t) ctx_pad, 64, (cuuint64_t) p.n_head_kv };
+        const cuuint64_t gdim[3] = { (cuuint64_t) a.T, 64, (cuuint64_t) p.n_head_kv };
         const cuuint64_t gstr[2] = { (cuuint64_t) ctx_pad * 2, (cuuint64_t) ctx_pad * 128 };
         const cuuint32_t box[3] = { 64, 64, 1 }, estr[3] = { 1, 1, 1 };
         const CUresult rc = get_encode()(&vmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void *) p.vt16, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,

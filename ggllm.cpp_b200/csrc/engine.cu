@@ -925,6 +925,17 @@ int b200_falcon_kv_read(b200_falcon * f, int layer, int pos, int n, float * k_ou
     if (v_out) B200_CUDA_CHECK(cudaMemcpy(v_out, f->v_cache + off, (size_t) n * row * 4, cudaMemcpyDeviceToHost));
     return 0;
 }
+// the fp16 shadow the prompt kernel reads (attention_ws.cu), positions [pos, pos + n) of `layer`: k16_out [n][n_head_kv][head_dim],
+// vt16_out [n_head_kv][head_dim][n].  The range may reach attention_ctx_pad(n_ctx), so that the padding columns can be inspected.
+int b200_falcon_kv_shadow_read(b200_falcon * f, int layer, int pos, int n, uint16_t * k16_out, uint16_t * vt16_out) {
+    const int ctx_pad = attention_ctx_pad(f->hp.n_ctx);
+    if (!f->k16 || layer < f->hp.layer_first || layer >= f->hp.layer_last || pos < 0 || n < 0 || pos + n > ctx_pad) return 1;
+    const size_t row = (size_t) f->HKV * f->D, lo = (size_t) (layer - f->hp.layer_first) * f->shadow_layer;
+    B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
+    if (k16_out && n) B200_CUDA_CHECK(cudaMemcpy(k16_out, f->k16 + lo + (size_t) pos * row, (size_t) n * row * 2, cudaMemcpyDeviceToHost));
+    if (vt16_out && n) B200_CUDA_CHECK(cudaMemcpy2D(vt16_out, (size_t) n * 2, f->vt16 + lo + pos, (size_t) ctx_pad * 2, (size_t) n * 2, row, cudaMemcpyDeviceToHost));
+    return 0;
+}
 int b200_falcon_kv_write(b200_falcon * f, int layer, int pos, int n, const float * k_in, const float * v_in) {
     if (layer < f->hp.layer_first || layer >= f->hp.layer_last || pos < 0 || n < 0 || pos + n > f->hp.n_ctx) return 1;
     const size_t row = (size_t) f->HKV * f->D, off = ((size_t) (layer - f->hp.layer_first) * f->hp.n_ctx + pos) * row;

@@ -208,6 +208,11 @@ int           b200_falcon_generate_greedy(b200_falcon * f, int32_t first_token, 
  * device-resident cache.  Return 0 on success, 1 if the layer is not on this rank or the range leaves [0, n_ctx). */
 int           b200_falcon_kv_read(b200_falcon * f, int layer, int pos, int n, float * k_out, float * v_out);
 int           b200_falcon_kv_write(b200_falcon * f, int layer, int pos, int n, const float * k_in, const float * v_in);
+/* the fp16 copy of the cache that prompt chunks of more than b200_mmv_max_n() tokens attend over (kept only when n_batch exceeds it):
+ * positions [pos, pos + n) of one layer as fp16 bit patterns, k16_out [n][n_head_kv][head_dim] and vt16_out [n_head_kv][head_dim][n]
+ * (V transposed; either may be NULL).  The range may extend past n_ctx to n_ctx rounded up to 64, the padding of the transposed copy.
+ * Return 0 on success, 1 if the engine keeps no such copy, the layer is not on this rank or the range is invalid. */
+int           b200_falcon_kv_shadow_read(b200_falcon * f, int layer, int pos, int n, uint16_t * k16_out, uint16_t * vt16_out);
 /* session file over the device KV cache (what falcon_save_session_file / falcon_load_session_file keep of the KV state,
  * libfalcon.cpp:4490-4563), in this library's own container: positions [0, n_tokens) of every local layer.  save: 0 / -1.
  * load: the number of positions restored (continue evaluating at that n_past), -1 on a missing / truncated / mismatching file. */
