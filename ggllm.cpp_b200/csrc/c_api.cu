@@ -128,6 +128,12 @@ void b200_actq_download(const b200_actq * a, int8_t * q, float * d, float * s, i
 
 int b200_mmv_max_n(void) { return 8; }
 
+int b200_mmv_launch_shape(int wtype, int64_t K, int mode, int * nt_j_d) {
+    const MmvShape s = mmv_fast_pick_shape(wtype, (int) K, mode);
+    if (nt_j_d) { nt_j_d[0] = s.nt; nt_j_d[1] = s.j; nt_j_d[2] = s.d; }
+    return s.nt ? 1 : 0;
+}
+
 void b200_mul_mat_vec_q(const b200_weight * w, const b200_actq * a, float * y, int64_t y_stride, int epilogue, const float * r1, const float * r2) {
     MmvEpilogue e = { epilogue, r1, r2 };
     launch_mmv(w->W, a->A, y, y_stride, e, g_stream);

@@ -344,7 +344,8 @@ bool launch_gemm_tc(const WPlanes & W, const __half * X, int64_t x_stride, int N
     // fewer than ~100 tiles cannot fill the 132 SMs of an H100: split K in two (deterministic, see GemmArgs::ksplit)
     const int tiles = (W.M + BM - 1) / BM * ((N + BN - 1) / BN);
     a.ksplit = (tiles < 100 && !epi_gelu && W.K / BK >= 8 && !getenv("B200_GEMM_NOSPLIT")) ? 2 : 1;
-    if (a.ksplit > 1) B200_CUDA_CHECK(cudaMemsetAsync(Y, 0, ((size_t) (N - 1) * y_stride + W.M) * sizeof(float), stream));
+    // the two halves add into Y: clear the N rows of M outputs, and only those (columns M .. y_stride-1 belong to the caller)
+    if (a.ksplit > 1) B200_CUDA_CHECK(cudaMemset2DAsync(Y, (size_t) y_stride * sizeof(float), 0, (size_t) W.M * sizeof(float), (size_t) N, stream));
     CUtensorMap map;
     const cuuint64_t gdim[2] = { (cuuint64_t) W.K, (cuuint64_t) N };
     const cuuint64_t gstr[1] = { (cuuint64_t) x_stride * 2 };

@@ -43,6 +43,8 @@ struct FastX {
     int l2_dist;                // set by the launcher: rows of HBM -> L2 prefetch ahead of the register ring
 };
 bool   launch_mmv_fast_x(const WPlanes & W, const FastX & X, float * y, int64_t y_stride, MmvEpilogue e, cudaStream_t stream);
+struct MmvShape { int nt, j, d; };                  // NT threads per CTA, J pieces per thread, ring depth D; nt == 0: generic kernel
+MmvShape mmv_fast_pick_shape(int wtype, int K, int mode);      // the shape launch_mmv_fast_x launches (B200_* switches included)
 bool   mmv_fast_supports(int wtype, int K, int mode);
 bool   mmv_fast_fills_sm(const WPlanes & W);       // its CTAs leave no registers for a side-stream kernel beside them
 // ---- ops.cu

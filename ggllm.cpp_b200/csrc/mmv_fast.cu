@@ -215,26 +215,49 @@ static void launch_cfg(const WPlanes & W, const FastX & X, float * y, int64_t y_
     } else B200_ASSERT(!"mmv_fast: this weight type takes quantised activations only (mode 0)");
 }
 
+// The launch shape (NT threads, J pieces per thread, ring depth D) for a row of K weights and activation mode `mode`;
+// nt == 0: not covered, the caller uses the generic ring kernel of mmv.cu
 template <int TYPE>
-static bool launch_type(const WPlanes & W, const FastX & X, float * y, int64_t y_stride, Epi epi, cudaStream_t stream) {
-    const int P = W.nb * FX<TYPE>::PPB;
-    if (W.K > 64 * 1024) return false;
-    if (X.mode == 2 && P > 512) return false;                 // the fused LayerNorm needs the whole row inside one CTA pass (J == 1)
+static MmvShape pick_shape_t(int K, int mode) {
+    const int P = K / (TYPE == T_Q4_0 ? 32 : 256) * FX<TYPE>::PPB;
+    if (K > 64 * 1024) return {};
+    if (mode == 2 && P > 512) return {};                      // the fused LayerNorm needs the whole row inside one CTA pass (J == 1)
     constexpr int D1 = FX<TYPE>::D256;                        // ring depth for one piece per thread; D * J stays constant
-    if (P <= 128 && D1 == 4) launch_cfg<TYPE, 128, 1, D1>(W, X, y, y_stride, epi, stream);       // 64-weight pieces (Q3_K): K = 8192 is 128 pieces
-    else if (P > 128 && P <= 160 && D1 == 8 && !getenv("B200_NO_NT160")) launch_cfg<TYPE, 160, 1, D1>(W, X, y, y_stride, epi, stream);   // Falcon-7B: K = 4544 is 142 pieces
-    else if (P <= 256) launch_cfg<TYPE, 256, 1, D1>(W, X, y, y_stride, epi, stream);
+    if (P <= 128 && D1 == 4) return { 128, 1, D1 };                                        // 64-weight pieces (Q3_K): K = 8192 is 128 pieces
+    if (P > 128 && P <= 160 && D1 == 8 && !getenv("B200_NO_NT160")) return { 160, 1, D1 }; // Falcon-7B: K = 4544 is 142 pieces
+    if (P <= 256) return { 256, 1, D1 };
     // Falcon-180B (K = 14848: 464 pieces): two 256-thread CTAs at 96 registers instead of one 512-thread CTA at 128 leave a quarter of the
     // register file to the attention kernels of the other stream, as the K = 8192 shape does
-    else if (P > 256 && P <= 512 && D1 == 8 && X.mode == 0 && !getenv("B200_NO_NT256J2")) launch_cfg<TYPE, 256, 2, D1 / 2>(W, X, y, y_stride, epi, stream);
-    else if (P <= 512) launch_cfg<TYPE, 512, 1, D1>(W, X, y, y_stride, epi, stream);
+    if (P > 256 && P <= 512 && D1 == 8 && mode == 0 && !getenv("B200_NO_NT256J2")) return { 256, 2, D1 / 2 };
+    if (P <= 512) return { 512, 1, D1 };
     // Falcon-7B's ffn_down (K = 18176: 568 pieces): 3 pieces per thread of a 192-thread CTA use 568 of 576 slots; the 512 x 2 shape
     // below would leave 45 % of its lanes without a piece (and its 128-register CTAs own the whole register file)
-    else if (P > 512 && P <= 576 && D1 == 8 && X.mode == 0 && !getenv("B200_NO_NT192")) launch_cfg<TYPE, 192, 3, 2>(W, X, y, y_stride, epi, stream);
-    else if (P <= 1024) launch_cfg<TYPE, 512, 2, D1 / 2>(W, X, y, y_stride, epi, stream);
-    else if (P <= 2048 && D1 == 8) launch_cfg<TYPE, 512, 4, 2>(W, X, y, y_stride, epi, stream);
-    else return false;
-    return true;
+    if (P > 512 && P <= 576 && D1 == 8 && mode == 0 && !getenv("B200_NO_NT192")) return { 192, 3, 2 };
+    if (P <= 1024) return { 512, 2, D1 / 2 };
+    if (P <= 2048 && D1 == 8) return { 512, 4, 2 };
+    return {};
+}
+
+MmvShape mmv_fast_pick_shape(int wtype, int K, int mode) {
+    switch (wtype) {
+        case T_Q4_K: return pick_shape_t<T_Q4_K>(K, mode);
+        case T_Q4_0: return pick_shape_t<T_Q4_0>(K, mode);
+        case T_Q3_K: return mode == 0 && !getenv("B200_Q3K_GENERIC") ? pick_shape_t<T_Q3_K>(K, mode) : MmvShape{};
+    }
+    return {};
+}
+
+template <int TYPE>
+static void launch_type(const MmvShape & s, const WPlanes & W, const FastX & X, float * y, int64_t y_stride, Epi epi, cudaStream_t stream) {
+    constexpr int D1 = FX<TYPE>::D256;
+    if (s.nt == 128) launch_cfg<TYPE, 128, 1, D1>(W, X, y, y_stride, epi, stream);
+    else if (s.nt == 160) launch_cfg<TYPE, 160, 1, D1>(W, X, y, y_stride, epi, stream);
+    else if (s.nt == 256 && s.j == 1) launch_cfg<TYPE, 256, 1, D1>(W, X, y, y_stride, epi, stream);
+    else if (s.nt == 256) launch_cfg<TYPE, 256, 2, D1 / 2>(W, X, y, y_stride, epi, stream);
+    else if (s.nt == 512 && s.j == 1) launch_cfg<TYPE, 512, 1, D1>(W, X, y, y_stride, epi, stream);
+    else if (s.nt == 192) launch_cfg<TYPE, 192, 3, 2>(W, X, y, y_stride, epi, stream);
+    else if (s.nt == 512 && s.j == 2) launch_cfg<TYPE, 512, 2, D1 / 2>(W, X, y, y_stride, epi, stream);
+    else launch_cfg<TYPE, 512, 4, 2>(W, X, y, y_stride, epi, stream);
 }
 
 // returns false if the shape / type is not covered (the caller then uses the generic ring kernel of mmv.cu)
@@ -250,12 +273,14 @@ bool launch_mmv_fast_x(const WPlanes & W, const FastX & X, float * y, int64_t y_
     if (dist_bytes < 0) { const char * s = getenv("B200_L2PF_KB"); dist_bytes = (s ? atoi(s) : 0) * 1024; }
     FastX Xp = X;
     Xp.l2_dist = W.stride[0] ? (int) (dist_bytes / W.stride[0]) : 0;
+    const MmvShape s = mmv_fast_pick_shape(W.type, W.K, X.mode);
+    if (!s.nt) return false;
     switch (W.type) {
-        case T_Q4_K: return launch_type<T_Q4_K>(W, Xp, y, y_stride, epi, stream);
-        case T_Q4_0: return launch_type<T_Q4_0>(W, Xp, y, y_stride, epi, stream);
-        case T_Q3_K: return X.mode == 0 && !getenv("B200_Q3K_GENERIC") && launch_type<T_Q3_K>(W, Xp, y, y_stride, epi, stream);
+        case T_Q4_K: launch_type<T_Q4_K>(s, W, Xp, y, y_stride, epi, stream); break;
+        case T_Q4_0: launch_type<T_Q4_0>(s, W, Xp, y, y_stride, epi, stream); break;
+        case T_Q3_K: launch_type<T_Q3_K>(s, W, Xp, y, y_stride, epi, stream); break;
     }
-    return false;
+    return true;
 }
 // Which (type, K, activation mode) the fused single-stream decode path of engine.cu may rely on.  Q3_K has a fast mat-vec
 // (used through launch_mmv) but is NOT listed: its kernel is issue-bound, and the two-stream per-node path, which runs the

@@ -102,6 +102,12 @@ int    b200_mul_mat_vec_q_chain(const b200_weight * w, const b200_actq * a_in, f
  * Returns 0 for a type without a device quantiser (quantise on the host then), 1 on success. */
 int    b200_quantize_weights(int ggml_type, const float * x_dev, void * blocks_dev, int64_t n_elems);
 int    b200_mmv_max_n(void);
+/* which kernel the decode mat-vec runs for a weight type, row length K and activation mode (0 quantised rows, as
+ * b200_mul_mat_vec_q / b200_mul_mat / b200_mul_mat_vec_q_chain; 1 fp32 row and 2 fp32 row + LayerNorm, as b200_mul_mat_vec_fused),
+ * with the B200_NO_NT160 / B200_NO_NT256J2 / B200_NO_NT192 / B200_Q3K_GENERIC switches of the current environment applied.
+ * Returns 1 and nt_j_d = {threads per CTA, pieces per thread, ring depth} for a tuned shape; 0 (nt_j_d = {0, 0, 0}) when the
+ * generic ring kernel runs, or for modes 1 / 2 when the fused entry points decline.  B200_MMV_GENERIC is not applied here. */
+int    b200_mmv_launch_shape(int ggml_type, int64_t K, int mode, int * nt_j_d);
 /* the GEMM half alone, on fp16 activations x[n][k] already on the device (what b200_mul_mat does after quantising):
  * impl 1 = wgmma tensor-core kernel (returns 0 if the shape is not covered: N > 512 or K % 64 != 0),
  * impl 0 = CUDA-core kernel with identical operand rounding (the test reference for impl 1). */
