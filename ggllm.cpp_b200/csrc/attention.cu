@@ -495,5 +495,5 @@ int launch_attention(const float * qkv, const float * k_cache, const float * v_c
     AttnParams pt = p; pt.trace = b200_trace_slot("attention");
     attention_kernel<<<grid, ATT_THREADS, smem, stream>>>(qkv, k_cache, v_cache, out, out_stride, pt);
     B200_CUDA_CHECK(cudaGetLastError());
-    return 1;
+    return p.fuse_rope ? 2 : 1;
 }

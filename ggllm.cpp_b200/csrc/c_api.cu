@@ -139,7 +139,7 @@ void b200_mul_mat_vec_q(const b200_weight * w, const b200_actq * a, float * y, i
     launch_mmv(w->W, a->A, y, y_stride, e, g_stream);
 }
 
-// scratch for the one-shot b200_mul_mat (quantised activations, fp16 operand, GEMM workspace); grows on demand
+// scratch for the one-shot b200_mul_mat (quantised activations, fp16 operand); grows on demand
 static void * g_scratch = nullptr; static size_t g_scratch_bytes = 0;
 static void * scratch(size_t bytes) {
     if (bytes > g_scratch_bytes) {
@@ -161,13 +161,12 @@ void b200_mul_mat(const b200_weight * w, const float * x, int64_t x_stride, int 
         MmvEpilogue e = { EPI_NONE, nullptr, nullptr };
         launch_mmv(W, A, y, y_stride, e, g_stream);
     } else {
-        const size_t hbytes = round_up((size_t) N * W.K * 2, 256), wsb = mmq_gemm_workspace_bytes(W, N);
-        uint8_t * base = (uint8_t *) scratch(abytes + hbytes + wsb);
+        uint8_t * base = (uint8_t *) scratch(abytes + (size_t) N * W.K * 2);
         ActQ A; actq_bind(A, at, W.K, N, base);
         launch_quantize_act(x, x_stride, A, g_stream);
         __half * xh = (__half *) (base + abytes);
         launch_actq_to_f16(A, xh, W.K, g_stream);
-        launch_mmq_gemm(W, xh, W.K, N, y, y_stride, 0, base + abytes + hbytes, wsb, g_stream);
+        launch_mmq_gemm(W, xh, W.K, N, y, y_stride, 0, g_stream);
     }
 }
 

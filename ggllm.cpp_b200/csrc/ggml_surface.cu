@@ -90,16 +90,15 @@ void op_mul_mat(const abi::tensor * src0, const abi::tensor * src1, abi::tensor 
     else {
         const int at = act_type_for(W.type);
         static void * act = nullptr; static size_t act_bytes = 0;
-        const size_t need = actq_bytes(at, W.K, N) + (N > b200_mmv_max_n() ? round_up((size_t) N * W.K * 2, 256) + mmq_gemm_workspace_bytes(W, N) : 0);
+        const size_t need = actq_bytes(at, W.K, N) + (N > b200_mmv_max_n() ? (size_t) N * W.K * 2 : 0);
         if (need > act_bytes) { if (act) { B200_CUDA_CHECK(cudaStreamSynchronize(g_st)); B200_CUDA_CHECK(cudaFree(act)); } act_bytes = round_up(need, 1 << 20); B200_CUDA_CHECK(cudaMalloc(&act, act_bytes)); }
         ActQ A; actq_bind(A, at, W.K, N, act);
         launch_quantize_act(x, W.K, A, g_st);
         if (N <= b200_mmv_max_n()) { MmvEpilogue e = { EPI_NONE, nullptr, nullptr }; launch_mmv(W, A, y, W.M, e, g_st); }
         else {
-            uint8_t * p = (uint8_t *) act + actq_bytes(at, W.K, N);
-            __half * xh = (__half *) p; p += round_up((size_t) N * W.K * 2, 256);
+            __half * xh = (__half *) ((uint8_t *) act + actq_bytes(at, W.K, N));
             launch_actq_to_f16(A, xh, W.K, g_st);
-            launch_mmq_gemm(W, xh, W.K, N, y, W.M, 0, p, mmq_gemm_workspace_bytes(W, N), g_st);
+            launch_mmq_gemm(W, xh, W.K, N, y, W.M, 0, g_st);
         }
     }
     dst->meta.cuda_perf_mal_mul_type = N <= b200_mmv_max_n() ? 1 : 16;        // device tag of --debug-timings (ggml.c:18266-18358)

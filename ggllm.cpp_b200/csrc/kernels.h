@@ -109,9 +109,7 @@ void   launch_attention_prefill(const float * qkv, const float * k_cache, const 
                                 const AttnParams & p, float * scratch, cudaStream_t stream);
 
 // ---- gemm.cu : Y[n][m] = sum_k W[m][k] * X[n][k], N large (prompt), wgmma tensor cores
-void   launch_mmq_gemm(const WPlanes & W, const __half * X, int64_t x_stride, int N, float * Y, int64_t y_stride,
-                       int epi_gelu, void * workspace, size_t workspace_bytes, cudaStream_t stream);
-size_t mmq_gemm_workspace_bytes(const WPlanes & W, int N);
+void   launch_mmq_gemm(const WPlanes & W, const __half * X, int64_t x_stride, int N, float * Y, int64_t y_stride, int epi_gelu, cudaStream_t stream);
 
 // ---- sampling.cu: the reference's default sampling chain on the device (repetition penalty, top-k, top-p, temperature, MT19937 draw)
 #define B200_SAMPLER_MAX_WINDOW 256
