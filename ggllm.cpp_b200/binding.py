@@ -19,12 +19,12 @@ PART_A = ["b200_event_create", "b200_event_destroy", "b200_event_record", "b200_
           "b200_weight_free", "b200_weight_device_bytes", "b200_dequantize_rows", "b200_actq_alloc", "b200_actq_free",
           "b200_quantize_act", "b200_actq_download", "b200_mul_mat", "b200_mul_mat_f16", "b200_mul_mat_vec_fused", "b200_mul_mat_vec_q", "b200_mul_mat_vec_q_chain", "b200_quantize_weights", "b200_mmv_max_n", "b200_mmv_launch_shape", "b200_layernorm",
           "b200_gelu", "b200_add", "b200_rope_neox", "b200_attention", "b200_layernorm_q", "b200_attention_decode",
-          "b200_sampler_create", "b200_sampler_sample", "b200_sampler_free"]
+          "b200_sampler_create", "b200_sampler_create_chain", "b200_sampler_sample", "b200_sampler_mirostat_mu", "b200_sampler_free"]
 PART_B = ["b200_falcon_create", "b200_falcon_set_tensor", "b200_falcon_set_tensor_random", "b200_falcon_load_ggcc",
           "b200_ggcc_read_hparams", "b200_falcon_free", "b200_falcon_weight_bytes", "b200_nccl_unique_id",
           "b200_falcon_init_pipeline", "b200_falcon_eval", "b200_falcon_decode_dev", "b200_falcon_logits_dev", "b200_falcon_generate_greedy",
           "b200_falcon_last_launches", "b200_attention_long_launches", "b200_falcon_last_ms", "b200_falcon_stream", "b200_falcon_profile_matvec",
-          "b200_falcon_kv_read", "b200_falcon_kv_write", "b200_falcon_kv_shadow_read", "b200_falcon_kv_fill_random", "b200_falcon_generate", "b200_falcon_load_seconds", "b200_falcon_save_kv", "b200_falcon_load_kv"]
+          "b200_falcon_kv_read", "b200_falcon_kv_write", "b200_falcon_kv_shadow_read", "b200_falcon_kv_fill_random", "b200_falcon_generate", "b200_falcon_generate_chain", "b200_falcon_load_seconds", "b200_falcon_save_kv", "b200_falcon_load_kv"]
 
 
 def build(verbose=False):
@@ -65,7 +65,9 @@ def lib():
             "b200_falcon_kv_shadow_read": (i32, [vp, i32, i32, i32, vp, vp]),
             "b200_falcon_kv_fill_random": (i32, [vp, i32, i32, C.c_uint64]),
             "b200_sampler_create": (vp, [vp, vp, i32]), "b200_sampler_sample": (i32, [vp, vp, i32]), "b200_sampler_free": (None, [vp]),
+            "b200_sampler_create_chain": (vp, [vp, vp, i32]), "b200_sampler_mirostat_mu": (f32, [vp]),
             "b200_falcon_generate": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, vp]),
+            "b200_falcon_generate_chain": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, vp]),
             "b200_falcon_load_seconds": (C.c_double, [vp, vp]),
             "b200_falcon_save_kv": (i32, [vp, C.c_char_p, i32]), "b200_falcon_load_kv": (i32, [vp, C.c_char_p]),
             "b200_falcon_create": (vp, [vp]), "b200_falcon_set_tensor": (None, [vp, C.c_char_p, i32, i32, vp, vp]),
@@ -222,18 +224,40 @@ class SamplingParams(C.Structure):
         super().__init__(top_k, top_p, temp, repeat_penalty, repeat_last_n, seed)
 
 
+class SamplingChain(C.Structure):
+    """b200_sampling_chain: falcon_main's whole chain with its defaults (examples/falcon_common.h:40-52); top_k <= 0 is the whole
+    vocabulary, logit_bias a {id: value} mapping (value may be -inf: falcon_main's --ignore-eos)"""
+    _fields_ = [("top_k", C.c_int32), ("top_p", C.c_float), ("tfs_z", C.c_float), ("typical_p", C.c_float), ("temp", C.c_float),
+                ("repeat_penalty", C.c_float), ("frequency_penalty", C.c_float), ("presence_penalty", C.c_float),
+                ("repeat_last_n", C.c_int32), ("mirostat", C.c_int32), ("mirostat_tau", C.c_float), ("mirostat_eta", C.c_float),
+                ("seed", C.c_uint32), ("n_logit_bias", C.c_int32), ("logit_bias_ids", C.c_void_p), ("logit_bias_values", C.c_void_p)]
+
+    def __init__(self, top_k=40, top_p=0.95, tfs_z=1.0, typical_p=1.0, temp=0.8, repeat_penalty=1.1, frequency_penalty=0.0,
+                 presence_penalty=0.0, repeat_last_n=64, mirostat=0, mirostat_tau=5.0, mirostat_eta=0.1, seed=1, logit_bias=None):
+        ids = np.array(list((logit_bias or {}).keys()), np.int32)
+        vals = np.array(list((logit_bias or {}).values()), np.float32)
+        self._bias = (ids, vals)                                    # kept alive with the struct
+        super().__init__(top_k, top_p, tfs_z, typical_p, temp, repeat_penalty, frequency_penalty, presence_penalty, repeat_last_n,
+                         mirostat, mirostat_tau, mirostat_eta, seed, ids.size, ids.ctypes.data if ids.size else None,
+                         vals.ctypes.data if vals.size else None)
+
+
 class Sampler:
-    """stand-alone device sampler over logits rows in HBM (b200_sampler_*)"""
+    """stand-alone device sampler over logits rows in HBM (b200_sampler_*); params: SamplingParams or SamplingChain"""
 
     def __init__(self, params, last_tokens=()):
         self.L = lib()
         lt = np.ascontiguousarray(last_tokens, dtype=np.int32)
-        self.h = self.L.b200_sampler_create(C.byref(params), _np_ptr(lt) if lt.size else None, lt.size)
+        create = self.L.b200_sampler_create_chain if isinstance(params, SamplingChain) else self.L.b200_sampler_create
+        self.h = create(C.byref(params), _np_ptr(lt) if lt.size else None, lt.size)
         if not self.h:
             raise ValueError("b200_sampler_create: bad sampling parameters")
 
     def sample(self, logits_dev_ptr, n_vocab):
         return int(self.L.b200_sampler_sample(self.h, logits_dev_ptr, n_vocab))
+
+    def mirostat_mu(self):
+        return float(self.L.b200_sampler_mirostat_mu(self.h))
 
     def free(self):
         if self.h:
@@ -324,6 +348,15 @@ class Falcon:
         rc = self.L.b200_falcon_generate(self.h, C.byref(params), _np_ptr(lt) if lt.size else None, lt.size, int(first_token), n_past, n_steps, n_ctx_rope, _np_ptr(out))
         if rc != 0:
             raise RuntimeError("b200_falcon_generate failed (rc=%d)" % rc)
+        return out
+
+    def generate_chain(self, chain, last_tokens, first_token, n_past, n_steps, n_ctx_rope=0):
+        """generation with the whole sampling chain on the device (b200_falcon_generate_chain; chain: SamplingChain)"""
+        out = np.zeros(n_steps, dtype=np.int32)
+        lt = np.ascontiguousarray(last_tokens, dtype=np.int32)
+        rc = self.L.b200_falcon_generate_chain(self.h, C.byref(chain), _np_ptr(lt) if lt.size else None, lt.size, int(first_token), n_past, n_steps, n_ctx_rope, _np_ptr(out))
+        if rc != 0:
+            raise RuntimeError("b200_falcon_generate_chain failed (rc=%d)" % rc)
         return out
 
     def decode_dev(self, token_dev_ptr, n_past, n_ctx_rope=0):

@@ -232,28 +232,72 @@ void b200_attention(float * qkv, float * kc, float * vc, float * out, int n_head
 }
 
 // ---- stand-alone sampler over a logits row on the device (the engine's generation loop runs the same kernel inside its step graph)
+// One sampler implementation: the default-chain parameters become a chain with every extra switched off.
+b200_sampling_chain sampler_chain_of(const b200_sampling_params & sp) {
+    b200_sampling_chain c{};
+    c.top_k = sp.top_k; c.top_p = sp.top_p; c.tfs_z = 1.0f; c.typical_p = 1.0f; c.temp = sp.temp;
+    c.repeat_penalty = sp.repeat_penalty; c.frequency_penalty = 0.0f; c.presence_penalty = 0.0f; c.repeat_last_n = sp.repeat_last_n;
+    c.mirostat = 0; c.mirostat_tau = 5.0f; c.mirostat_eta = 0.1f; c.seed = sp.seed; c.n_logit_bias = 0;
+    return c;
+}
+// validates a chain (n_vocab < 0: bias ids not checked against a vocabulary yet) and converts it to the kernel's parameters
+bool sampler_params_of(const b200_sampling_chain * c, int n_vocab, SamplerParams * out) {
+    if (!c || c->repeat_last_n < 0 || c->repeat_last_n > B200_SAMPLER_MAX_WINDOW || c->mirostat < 0 || c->mirostat > 2) return false;
+    for (float v : { c->top_p, c->tfs_z, c->typical_p, c->temp, c->repeat_penalty, c->frequency_penalty, c->presence_penalty,
+                     c->mirostat_tau, c->mirostat_eta })
+        if (v != v) return false;
+    if (c->n_logit_bias < 0 || c->n_logit_bias > B200_SAMPLER_MAX_BIAS || (c->n_logit_bias > 0 && (!c->logit_bias_ids || !c->logit_bias_values))) return false;
+    SamplerParams p;
+    memset(&p, 0, sizeof(p));                                        // memcmp-comparable (the engine rebuilds its graph on a change)
+    p.top_k = c->top_k; p.top_p = c->top_p; p.temp = c->temp; p.repeat_penalty = c->repeat_penalty;
+    p.tfs_z = c->tfs_z; p.typical_p = c->typical_p; p.frequency_penalty = c->frequency_penalty; p.presence_penalty = c->presence_penalty;
+    p.mirostat = c->mirostat; p.mirostat_tau = c->mirostat_tau; p.mirostat_eta = c->mirostat_eta;
+    p.n_bias = c->n_logit_bias;
+    for (int i = 0; i < p.n_bias; i++) {
+        const int32_t id = c->logit_bias_ids[i];
+        if (id < 0 || (n_vocab >= 0 && id >= n_vocab)) return false;
+        for (int j = 0; j < i; j++) if (c->logit_bias_ids[j] == id) return false;
+        if (c->logit_bias_values[i] != c->logit_bias_values[i]) return false;
+        p.bias_id[i] = id; p.bias_value[i] = c->logit_bias_values[i];
+    }
+    *out = p;
+    return true;
+}
 struct b200_sampler { SamplerState * st; SamplerParams p; float * work; size_t work_floats; int32_t * out; };
-b200_sampler * b200_sampler_create(const b200_sampling_params * sp, const int32_t * last_tokens, int n_last) {
-    if (!sp || sp->top_k < 1 || sp->top_k > 1024 || sp->repeat_last_n < 0 || sp->repeat_last_n > B200_SAMPLER_MAX_WINDOW || n_last < 0) return nullptr;
+b200_sampler * b200_sampler_create_chain(const b200_sampling_chain * c, const int32_t * last_tokens, int n_last) {
+    SamplerParams p;
+    if (!sampler_params_of(c, -1, &p) || n_last < 0 || (n_last > 0 && !last_tokens)) return nullptr;
     b200_sampler * s = new b200_sampler();
-    s->st = sampler_state_alloc(); s->p = { sp->top_k, sp->top_p, sp->temp, sp->repeat_penalty }; s->work = nullptr; s->work_floats = 0;
+    s->st = sampler_state_alloc(); s->p = p; s->work = nullptr; s->work_floats = 0;
     B200_CUDA_CHECK(cudaMalloc(&s->out, 4));
     int32_t * w = nullptr;
     if (n_last > 0) { B200_CUDA_CHECK(cudaMalloc(&w, (size_t) n_last * 4)); B200_CUDA_CHECK(cudaMemcpyAsync(w, last_tokens, (size_t) n_last * 4, cudaMemcpyHostToDevice, g_stream)); }
-    launch_sampler_init(s->st, sp->seed, w, n_last, sp->repeat_last_n, g_stream);
+    launch_sampler_init(s->st, c->seed, w, n_last, c->repeat_last_n, 2.0f * c->mirostat_tau, g_stream);
     B200_CUDA_CHECK(cudaStreamSynchronize(g_stream));
     if (w) B200_CUDA_CHECK(cudaFree(w));
     return s;
 }
+b200_sampler * b200_sampler_create(const b200_sampling_params * sp, const int32_t * last_tokens, int n_last) {
+    if (!sp || sp->top_k < 1 || sp->top_k > 1024 || sp->repeat_last_n < 0 || sp->repeat_last_n > B200_SAMPLER_MAX_WINDOW || n_last < 0) return nullptr;
+    const b200_sampling_chain c = sampler_chain_of(*sp);
+    return b200_sampler_create_chain(&c, last_tokens, n_last);
+}
 int32_t b200_sampler_sample(b200_sampler * s, const float * logits_dev, int n_vocab) {
-    if ((size_t) n_vocab > s->work_floats) { if (s->work) B200_CUDA_CHECK(cudaFree(s->work)); s->work_floats = (size_t) n_vocab; B200_CUDA_CHECK(cudaMalloc(&s->work, s->work_floats * 4)); }
-    if (s->p.top_k > n_vocab) s->p.top_k = n_vocab;
-    launch_sample(logits_dev, n_vocab, s->p, s->st, s->work, s->out, nullptr, nullptr, g_stream);
+    if (n_vocab <= 0) return -1;
+    for (int i = 0; i < s->p.n_bias; i++) if (s->p.bias_id[i] >= n_vocab) return -1;      // never written outside the row
+    if (sampler_work_floats(n_vocab) > s->work_floats) {
+        if (s->work) B200_CUDA_CHECK(cudaFree(s->work));
+        s->work_floats = sampler_work_floats(n_vocab); B200_CUDA_CHECK(cudaMalloc(&s->work, s->work_floats * 4));
+    }
+    SamplerParams p = s->p;
+    if (p.top_k > n_vocab) p.top_k = n_vocab;
+    launch_sample(logits_dev, n_vocab, p, s->st, s->work, s->out, nullptr, nullptr, g_stream);
     int32_t id = -1;
     B200_CUDA_CHECK(cudaMemcpyAsync(&id, s->out, 4, cudaMemcpyDeviceToHost, g_stream));
     B200_CUDA_CHECK(cudaStreamSynchronize(g_stream));
     return id;
 }
+float b200_sampler_mirostat_mu(const b200_sampler * s) { B200_CUDA_CHECK(cudaStreamSynchronize(g_stream)); return sampler_mu(s->st); }
 void b200_sampler_free(b200_sampler * s) { if (!s) return; sampler_state_free(s->st); cudaFree(s->work); cudaFree(s->out); delete s; }
 
 // the decode step's LayerNorm node exactly as the engine launches it (cluster kernel for one row of <= 8192 values, register

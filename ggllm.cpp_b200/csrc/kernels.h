@@ -111,13 +111,23 @@ void   launch_attention_prefill(const float * qkv, const float * k_cache, const 
 // ---- gemm.cu : Y[n][m] = sum_k W[m][k] * X[n][k], N large (prompt), wgmma tensor cores
 void   launch_mmq_gemm(const WPlanes & W, const __half * X, int64_t x_stride, int N, float * Y, int64_t y_stride, int epi_gelu, cudaStream_t stream);
 
-// ---- sampling.cu: the reference's default sampling chain on the device (repetition penalty, top-k, top-p, temperature, MT19937 draw)
+// ---- sampling.cu: falcon_main's sampling chain on the device (logit bias, repetition / frequency / presence penalties, top-k,
+// tail-free, typical, top-p, temperature, mirostat 1 / 2, MT19937 draw)
 #define B200_SAMPLER_MAX_WINDOW 256
-struct SamplerParams { int top_k; float top_p; float temp; float repeat_penalty; };
+#define B200_SAMPLER_MAX_BIAS 64
+struct SamplerParams {
+    int top_k;                          // <= 0: whole vocabulary (1..1024: block arg-max rounds, otherwise a radix sort of the row)
+    float top_p; float temp; float repeat_penalty;
+    float tfs_z, typical_p, frequency_penalty, presence_penalty;
+    int mirostat; float mirostat_tau, mirostat_eta;
+    int n_bias; int32_t bias_id[B200_SAMPLER_MAX_BIAS]; float bias_value[B200_SAMPLER_MAX_BIAS];   // unused entries zero (memcmp-comparable)
+};
 struct SamplerState;
 SamplerState * sampler_state_alloc();
 void   sampler_state_free(SamplerState * s);
-void   launch_sampler_init(SamplerState * s, uint32_t seed, const int32_t * window_dev, int n, int cap, cudaStream_t stream);
+size_t sampler_work_floats(int n_vocab);                       // size of launch_sample's `work` scratch
+float  sampler_mu(const SamplerState * s);                     // synchronous read of the mirostat state
+void   launch_sampler_init(SamplerState * s, uint32_t seed, const int32_t * window_dev, int n, int cap, float mu, cudaStream_t stream);
 void   launch_sample(const float * logits, int n_vocab, const SamplerParams & p, SamplerState * st, float * work, int32_t * out, int32_t * hist, int * step, cudaStream_t stream);
 
 // ---- engine.cu (internal, C++ linkage): adopt a matrix that is already resident in the planar layout (no copy, not freed by the engine)
