@@ -17,7 +17,7 @@ PART_A = ["b200_event_create", "b200_event_destroy", "b200_event_record", "b200_
           "b200_stream_synchronize", "b200_init", "b200_device_count", "b200_set_stream", "b200_synchronize", "b200_malloc", "b200_free", "b200_memcpy_h2d",
           "b200_memcpy_d2h", "b200_memset", "b200_host_malloc", "b200_host_free", "b200_weight_upload", "b200_weight_random",
           "b200_weight_free", "b200_weight_device_bytes", "b200_dequantize_rows", "b200_actq_alloc", "b200_actq_free",
-          "b200_quantize_act", "b200_actq_download", "b200_mul_mat", "b200_mul_mat_f16", "b200_mul_mat_vec_fused", "b200_mul_mat_vec_q", "b200_mul_mat_vec_q_chain", "b200_quantize_weights", "b200_mmv_max_n", "b200_mmv_launch_shape", "b200_layernorm",
+          "b200_quantize_act", "b200_actq_download", "b200_actq_alloc_f16", "b200_actq_download_f16", "b200_actq_to_f16", "b200_mul_mat", "b200_mul_mat_f16", "b200_mul_mat_vec_fused", "b200_mul_mat_vec_q", "b200_mul_mat_vec_q_chain", "b200_quantize_weights", "b200_mmv_max_n", "b200_mmv_launch_shape", "b200_layernorm",
           "b200_gelu", "b200_add", "b200_rope_neox", "b200_attention", "b200_layernorm_q", "b200_attention_decode",
           "b200_sampler_create", "b200_sampler_create_chain", "b200_sampler_sample", "b200_sampler_mirostat_mu", "b200_sampler_free"]
 PART_B = ["b200_falcon_create", "b200_falcon_set_tensor", "b200_falcon_set_tensor_random", "b200_falcon_load_ggcc",
@@ -54,6 +54,7 @@ def lib():
             "b200_dequantize_rows": (None, [vp, vp, i32, vp, i64]),
             "b200_actq_alloc": (vp, [i32, i64, i32]), "b200_actq_free": (None, [vp]), "b200_quantize_act": (None, [vp, i64, vp]),
             "b200_actq_download": (None, [vp, vp, vp, vp, vp]),
+            "b200_actq_alloc_f16": (vp, [i32, i64, i32]), "b200_actq_download_f16": (None, [vp, vp]), "b200_actq_to_f16": (None, [vp, vp, i64]),
             "b200_mul_mat": (None, [vp, vp, i64, i32, vp, i64]), "b200_mul_mat_vec_q": (None, [vp, vp, vp, i64, i32, vp, vp]),
             "b200_mmv_max_n": (i32, []), "b200_mmv_launch_shape": (i32, [i32, i64, i32, vp]),"b200_mul_mat_vec_fused": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, i32]), "b200_mul_mat_vec_q_chain": (i32, [vp, vp, vp, i32, vp]), "b200_quantize_weights": (i32, [i32, vp, vp, i64]), "b200_mul_mat_f16": (i32, [vp, vp, i64, i32, vp, i64, i32, i32]),
             "b200_layernorm": (None, [vp, i64, vp, vp, vp, i64, i32, i32]), "b200_gelu": (None, [vp, vp, i64]), "b200_add": (None, [vp, vp, vp, i64]),
@@ -186,10 +187,12 @@ class Weight:
 
 
 class ActQ:
-    def __init__(self, wtype, K, N):
+    """quantised activation rows; f16=True adds the fp16 GEMM-operand plane fp16(d * q) that every producer then fills too"""
+
+    def __init__(self, wtype, K, N, f16=False):
         self.L = lib()
         self.wtype, self.K, self.N = wtype, K, N
-        self.h = self.L.b200_actq_alloc(wtype, K, N)
+        self.h = (self.L.b200_actq_alloc_f16 if f16 else self.L.b200_actq_alloc)(wtype, K, N)
 
     def quantize(self, x_dev, x_stride=None):
         self.L.b200_quantize_act(x_dev, x_stride or self.K, self.h)
@@ -203,6 +206,16 @@ class ActQ:
         bs = np.empty((self.N, self.K // (16 if kq else 32)), np.int16)
         self.L.b200_actq_download(self.h, _np_ptr(q), _np_ptr(d), _np_ptr(s), _np_ptr(bs))
         return q, d, s, bs
+
+    def download_f16(self):
+        """-> the fp16 plane [N][K] (the ActQ must have been made with f16=True)"""
+        h = np.empty((self.N, self.K), np.float16)
+        self.L.b200_actq_download_f16(self.h, _np_ptr(h))
+        return h
+
+    def to_f16(self, buf, stride=None):
+        """fp16(d * q) of the codes and scales into the DevBuf `buf` [N][stride] (actq_to_f16: the GEMM operand built separately)"""
+        self.L.b200_actq_to_f16(self.h, buf.ptr, stride or self.K)
 
     def free(self):
         if self.h:

@@ -3,7 +3,7 @@
 // This is the INIT pass of the CPU mat-mul (ggml_compute_forward_mul_mat_q_f32, ggml.c:11462-11476), which the
 // reference CUDA kernels skip (they multiply fp32 activations).  Reproducing it makes the GPU mat-vec compute the
 // same integer block dots as the CPU oracle, and shrinks the activation tile staged in shared memory 4x.
-// Codes and scales are bit-exact with the CPU (tests/test_actquant_gpu.py):
+// Codes and scales are bit-exact with the CPU (tests/test_actq_edges_gpu.py, on ties, half-way products and clamps):
 //   Q8_K : quantize_row_q8_K_reference, k_quants.c:899-934 (iscale = -128/max, round-half-even, min(127,.))
 //   Q8_0 : the AVX/AVX2 body an x86 host runs, ggml.c:1201-1237 (id = 127/amax, round-half-even, d -> fp16)
 //   Q8_1 : ggml.c:1421-1470 (same, d kept in fp32, s = d * sum(q))

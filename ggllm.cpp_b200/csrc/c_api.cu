@@ -6,7 +6,7 @@
 #include <vector>
 
 struct b200_weight { WPlanes W; };
-struct b200_actq { ActQ A; void * base; size_t bytes; };
+struct b200_actq { ActQ A; void * base; size_t bytes; __half * h; };
 
 static cudaStream_t g_own_stream = nullptr;
 static cudaStream_t g_stream = nullptr;
@@ -113,9 +113,22 @@ b200_actq * b200_actq_alloc(int wtype, int64_t K, int N) {
     a->bytes = actq_bytes(at, (int) K, N);
     B200_CUDA_CHECK(cudaMalloc(&a->base, a->bytes));
     actq_bind(a->A, at, (int) K, N, a->base);
+    a->h = nullptr;
     return a;
 }
-void b200_actq_free(b200_actq * a) { if (a) { B200_CUDA_CHECK(cudaFree(a->base)); delete a; } }
+b200_actq * b200_actq_alloc_f16(int wtype, int64_t K, int N) {
+    b200_actq * a = b200_actq_alloc(wtype, K, N);
+    B200_CUDA_CHECK(cudaMalloc(&a->h, (size_t) N * K * sizeof(__half)));
+    a->A.h = a->h;
+    return a;
+}
+void b200_actq_free(b200_actq * a) { if (a) { B200_CUDA_CHECK(cudaFree(a->base)); if (a->h) B200_CUDA_CHECK(cudaFree(a->h)); delete a; } }
+void b200_actq_download_f16(const b200_actq * a, uint16_t * h) {
+    B200_ASSERT(a->h);
+    B200_CUDA_CHECK(cudaStreamSynchronize(g_stream));
+    B200_CUDA_CHECK(cudaMemcpy(h, a->h, (size_t) a->A.N * a->A.K * sizeof(__half), cudaMemcpyDeviceToHost));
+}
+void b200_actq_to_f16(const b200_actq * a, void * dst, int64_t dst_stride) { launch_actq_to_f16(a->A, (__half *) dst, dst_stride, g_stream); }
 void b200_quantize_act(const float * x, int64_t x_stride, b200_actq * a) { launch_quantize_act(x, x_stride, a->A, g_stream); }
 void b200_actq_download(const b200_actq * a, int8_t * q, float * d, float * s, int16_t * bs) {
     const ActQ & A = a->A; const int blk = act_block(A.type);

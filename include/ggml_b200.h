@@ -74,6 +74,13 @@ void        b200_actq_free(b200_actq * a);
 void        b200_quantize_act(const float * x_dev, int64_t x_stride, b200_actq * a);
 /* test hook: copy out codes q[N*K], scales d[N*K/blk], Q8_1 sums s[N*K/32] (or NULL), block sums bs (or NULL) */
 void        b200_actq_download(const b200_actq * a, int8_t * q, float * d, float * s, int16_t * bs);
+/* test hooks for the prompt GEMM's fp16 operand, fp16(d * q) per value (what the GEMM path multiplies):
+ * alloc_f16  : b200_actq_alloc plus an fp16 plane [N][K] that every producer writing `a` fills alongside the codes;
+ * download_f16: copy that plane out as fp16 bit patterns (a must come from b200_actq_alloc_f16);
+ * to_f16     : build the same operand from a's codes and scales into dst_dev [N][dst_stride] fp16 on the device. */
+b200_actq * b200_actq_alloc_f16(int weight_ggml_type, int64_t K, int N);
+void        b200_actq_download_f16(const b200_actq * a, uint16_t * h);
+void        b200_actq_to_f16(const b200_actq * a, void * dst_dev, int64_t dst_stride);
 
 /* ---- y[n][m] = sum_k W[m][k] x[n][k].  Replaces ggml_cuda_mul_mat (ggml-cuda.cu:2931-2951):
  * N == 1..b200_mmv_max_n(): fused dequantise + integer-dot mat-vec (replaces dequantize_mul_mat_vec*,

@@ -48,7 +48,11 @@ def test_activation_quantization_bit_exact(gpu, orc, t):
     rng = np.random.default_rng(11)
     x = rng.standard_normal((N, K)).astype(np.float32) * np.array([1, 10, 0.01, 100, 1], np.float32)[:, None]
     x[4, :256] = 0.0                      # an all-zero block
-    x[4, 300] = -x[4, 301]                # +/- tie on the block maximum: first one wins
+    x[4, 300], x[4, 301] = 5.0, -5.0      # +/- tie on the block maximum: first one wins
+    for blk in (32, 256):                 # the pair is the maximum magnitude of its 32-block and of its 256-block
+        b0 = 300 // blk * blk
+        a = np.abs(x[4, b0:b0 + blk])
+        assert list(np.flatnonzero(a == a.max()) + b0) == [300, 301]
     xd = gpu.DevBuf(src=x)
     A = gpu.ActQ(t, K, N)
     A.quantize(xd.ptr)
