@@ -439,10 +439,9 @@ bool launch_attention_long(const float * qkv, const float * k_cache, const float
     a.fuse_rope = p.fuse_rope; a.theta_scale = p.rope_theta_scale; a.kc_w = const_cast<float *>(k_cache); a.vc_w = const_cast<float *>(v_cache);
     a.k16 = p.k16; a.vt16 = p.vt16; a.ctx_pad = attention_ctx_pad(p.n_ctx);
     // one wave: as many key splits as SMs divided by the (KV head, head group) pairs -- Falcon-40B 18, 180B 9, 7B 29
-    static int sms = 0, force = -1;
-    if (!sms) { int dev; B200_CUDA_CHECK(cudaGetDevice(&dev)); B200_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)); }
+    static int force = -1;
     if (force < 0) { const char * e = getenv("B200_ATTN_SPLITS"); force = e ? atoi(e) : 0; }
-    a.n_splits = force > 0 ? force : sms / (p.n_head_kv * groups);
+    a.n_splits = force > 0 ? force : num_sms() / (p.n_head_kv * groups);
     a.n_splits = a.n_splits < 4 ? 4 : a.n_splits > AL_MAX_SPLITS ? AL_MAX_SPLITS : a.n_splits;
     // Q8_K blocks are 256 outputs = 4 heads: they must not straddle the 16-head groups the CTAs combine
     a.has_q = p.qout != nullptr && (p.qout->type != T_Q8_K || G % 4 == 0);

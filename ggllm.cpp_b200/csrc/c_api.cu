@@ -141,8 +141,8 @@ void b200_actq_download(const b200_actq * a, int8_t * q, float * d, float * s, i
 
 int b200_mmv_max_n(void) { return 8; }
 
-int b200_mmv_launch_shape(int wtype, int64_t K, int mode, int * nt_j_d) {
-    const MmvShape s = mmv_fast_pick_shape(wtype, (int) K, mode);
+int b200_mmv_launch_shape(int wtype, int64_t K, int * nt_j_d) {
+    const MmvShape s = mmv_fast_pick_shape(wtype, (int) K);
     if (nt_j_d) { nt_j_d[0] = s.nt; nt_j_d[1] = s.j; nt_j_d[2] = s.d; }
     return s.nt ? 1 : 0;
 }
@@ -183,17 +183,9 @@ void b200_mul_mat(const b200_weight * w, const float * x, int64_t x_stride, int 
     }
 }
 
-// y = W * Q(LayerNorm((ra + rb) + x) * gamma + beta)   (gamma == NULL: y = W * Q(x)), N = 1: the fused decode mat-vec
-int b200_mul_mat_vec_fused(const b200_weight * w, const float * x, const float * ra, const float * rb, const float * gamma, const float * beta,
-                           float * x_out, float * y, int epilogue) {
-    FastX X{}; X.mode = gamma ? 2 : 1; X.N = 1; X.x = x; X.x_stride = w->W.K; X.ra = ra; X.rb = rb; X.gamma = gamma; X.beta = beta; X.x_out = x_out;
-    MmvEpilogue e = { epilogue, nullptr, nullptr };
-    return launch_mmv_fast_x(w->W, X, y, w->W.M, e, g_stream) ? 1 : 0;
-}
-
 int b200_mul_mat_vec_q_chain(const b200_weight * w, const b200_actq * a_in, float * y, int epilogue, b200_actq * a_out) {
     const WPlanes & W = w->W;
-    if (!mmv_fast_supports(W.type, W.K, 0) || W.M % 256 != 0 || a_in->A.N != 1 || a_out->A.K != W.M) return 0;
+    if (!mmv_fast_supports(W.type, W.K) || W.M % 256 != 0 || a_in->A.N != 1 || a_out->A.K != W.M) return 0;
     if (a_out->A.type != T_Q8_K && a_out->A.type != T_Q8_0) return 0;
     static unsigned * ctr = nullptr; static int ctr_n = 0;
     if (ctr_n < W.M / 256) {
@@ -202,8 +194,7 @@ int b200_mul_mat_vec_q_chain(const b200_weight * w, const b200_actq * a_in, floa
     }
     ActQ out = a_out->A; out.N = 1;
     MmvEpilogue e = { epilogue, nullptr, nullptr, &out, ctr };
-    FastX X{}; X.mode = 0; X.N = 1; X.A = a_in->A;
-    return launch_mmv_fast_x(W, X, y, W.M, e, g_stream) ? 1 : 0;
+    return launch_mmv_fast(W, a_in->A, y, W.M, e, g_stream) ? 1 : 0;
 }
 
 int b200_mul_mat_f16(const b200_weight * w, const void * x_f16, int64_t x_stride, int N, float * y, int64_t y_stride, int epi_gelu, int impl) {

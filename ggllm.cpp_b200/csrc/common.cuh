@@ -39,6 +39,13 @@ static inline size_t round_up(size_t v, size_t a) { return (v + a - 1) / a * a; 
 // mat-vec of the other stream to drain.  25 % of the H100's 228 KB = 57 KB shared, rest L1.
 #define B200_CARVEOUT 25
 
+// multiprocessors of the current device (queried once): the persistent kernels size their grids by it
+inline int num_sms() {
+    static int n = 0;
+    if (!n) { int dev; B200_CUDA_CHECK(cudaGetDevice(&dev)); B200_CUDA_CHECK(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev)); }
+    return n;
+}
+
 #ifdef __CUDACC__
 
 // streaming 16-byte load of weight data: read-only path, do not allocate in L1 (each byte is used once)
@@ -87,6 +94,22 @@ __device__ __forceinline__ int dp4a_us(unsigned a, int b, int c) {              
     int d;
     asm("dp4a.u32.s32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
     return d;
+}
+// u8 x s8 dot of 16 weight bytes (four words) with 16 activation codes
+__device__ __forceinline__ int dot16(const uint32_t w0, const uint32_t w1, const uint32_t w2, const uint32_t w3, const uint4 x) {
+    int s = dp4a_us(w0, (int) x.x, 0); s = dp4a_us(w1, (int) x.y, s); s = dp4a_us(w2, (int) x.z, s); return dp4a_us(w3, (int) x.w, s);
+}
+// c + the two s16 halves of pair16 times the low (lo) or high (hi) two bytes of `bytes`, unsigned (us) or signed (ss)
+__device__ __forceinline__ int dp2a_lo_us(int pair16, uint32_t bytes, int c) { int d; asm("dp2a.lo.s32.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(pair16), "r"(bytes), "r"(c)); return d; }
+__device__ __forceinline__ int dp2a_hi_us(int pair16, uint32_t bytes, int c) { int d; asm("dp2a.hi.s32.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(pair16), "r"(bytes), "r"(c)); return d; }
+__device__ __forceinline__ int dp2a_lo_ss(int pair16, uint32_t bytes, int c) { int d; asm("dp2a.lo.s32.s32 %0, %1, %2, %3;" : "=r"(d) : "r"(pair16), "r"(bytes), "r"(c)); return d; }
+__device__ __forceinline__ int dp2a_hi_ss(int pair16, uint32_t bytes, int c) { int d; asm("dp2a.hi.s32.s32 %0, %1, %2, %3;" : "=r"(d) : "r"(pair16), "r"(bytes), "r"(c)); return d; }
+
+// fp16-LUT GELU (ggml.c:3461-3484, table 4281-4290): table_gelu_f16[f16(v)] = f16 of the fp32 formula at the fp16 input
+__device__ __forceinline__ float gelu_f16lut(float v) {
+    const float f = __half2float(__float2half_rn(v));
+    const float g = 0.5f * f * (1.0f + tanhf(0.79788456080286535587989211986876f * f * (1.0f + 0.044715f * f * f)));
+    return __half2float(__float2half_rn(g));
 }
 
 // ---- mbarrier + 1-D bulk (TMA) copy global -> shared: used to stage activation tiles ----

@@ -619,8 +619,8 @@ static void enqueue_attention(b200_falcon * f, int l, const AttnParams & ap, flo
 static bool fused_decode_ok(const b200_falcon * f) {
     if (getenv("B200_NO_FUSED_DECODE")) return false;
     for (const auto & L : f->layers)
-        if (!mmv_fast_supports(L.wo.type, L.wo.K, 0) || !mmv_fast_supports(L.down.type, L.down.K, 0) ||
-            !mmv_fast_supports(L.up.type, L.up.K, 0) || !mmv_fast_supports(L.wqkv.type, L.wqkv.K, 0)) return false;
+        if (!mmv_fast_supports(L.wo.type, L.wo.K) || !mmv_fast_supports(L.down.type, L.down.K) ||
+            !mmv_fast_supports(L.up.type, L.up.K) || !mmv_fast_supports(L.wqkv.type, L.wqkv.K)) return false;
     return f->act_type >= 0 && f->FF % 256 == 0;
 }
 // ---- decode (N == 1) on the register-resident mat-vecs, 7 kernels per layer: one LayerNorm kernel (the previous layer's residual adds +

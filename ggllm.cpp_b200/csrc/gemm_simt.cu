@@ -44,8 +44,7 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(const WPlanes W, const _
             const int m = m0 + tx * 4 + i;
             if (m < W.M) {
                 float v = acc[j][i];
-                if (epi_gelu) { const float f = __half2float(__float2half_rn(v));
-                    v = __half2float(__float2half_rn(0.5f * f * (1.0f + tanhf(0.79788456080286535587989211986876f * f * (1.0f + 0.044715f * f * f))))); }
+                if (epi_gelu) v = gelu_f16lut(v);
                 Y[(size_t) n * y_stride + m] = v;
             }
         }

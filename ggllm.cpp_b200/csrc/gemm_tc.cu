@@ -291,8 +291,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_tc_kernel(const __grid_consta
                     const int n = n0 + 8 * j + 2 * (lane & 3) + e;
                     if (n >= a.N) continue;
                     float y = acc[4 * j + 2 * i + e];
-                    if (a.epi_gelu) { const float f = __half2float(__float2half_rn(y));
-                        y = __half2float(__float2half_rn(0.5f * f * (1.0f + tanhf(0.79788456080286535587989211986876f * f * (1.0f + 0.044715f * f * f))))); }
+                    if (a.epi_gelu) y = gelu_f16lut(y);
                     if (a.ksplit > 1) atomicAdd(a.Y + (size_t) n * a.y_stride + m, y);
                     else a.Y[(size_t) n * a.y_stride + m] = y;
                 }

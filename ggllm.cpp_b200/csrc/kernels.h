@@ -31,21 +31,11 @@ struct MmvEpilogue { int kind; const float * r1; const float * r2;         // AD
 void   launch_mmv(const WPlanes & W, const ActQ & A, float * y, int64_t y_stride, MmvEpilogue epi, cudaStream_t stream);
 void   launch_mmv_f(const WPlanes & W, const float * x, int64_t x_stride, int N, float * y, int64_t y_stride, cudaStream_t stream); // f16/f32 weights
 
-// mmv_fast.cu: the tuned kernel (Q4_K, Q4_0) can take its activation row in three forms, see FastX there
-struct FastX {
-    int mode;                   // 0 quantised ActQ | 1 fp32 row, quantised in the prologue | 2 fp32 row, [+residuals] + LayerNorm + quantise in the prologue
-    int N;                      // activation rows (columns of Y)
-    ActQ A;                     // mode 0
-    const float * x; int64_t x_stride;          // modes 1, 2
-    const float * ra, * rb;     // mode 2, optional: x = (ra + rb) + x first
-    const float * gamma, * beta;
-    float * x_out;              // mode 2, optional: CTA 0 stores the updated x here
-    int l2_dist;                // set by the launcher: rows of HBM -> L2 prefetch ahead of the register ring
-};
-bool   launch_mmv_fast_x(const WPlanes & W, const FastX & X, float * y, int64_t y_stride, MmvEpilogue e, cudaStream_t stream);
+// mmv_fast.cu: the tuned kernel (Q4_K, Q4_0, Q3_K); false = type / K not covered, nothing launched
+bool   launch_mmv_fast(const WPlanes & W, const ActQ & A, float * y, int64_t y_stride, MmvEpilogue e, cudaStream_t stream);
 struct MmvShape { int nt, j, d; };                  // NT threads per CTA, J pieces per thread, ring depth D; nt == 0: generic kernel
-MmvShape mmv_fast_pick_shape(int wtype, int K, int mode);      // the shape launch_mmv_fast_x launches (B200_* switches included)
-bool   mmv_fast_supports(int wtype, int K, int mode);
+MmvShape mmv_fast_pick_shape(int wtype, int K);     // the shape launch_mmv_fast launches (B200_* switches included)
+bool   mmv_fast_supports(int wtype, int K);
 bool   mmv_fast_fills_sm(const WPlanes & W);       // its CTAs leave no registers for a side-stream kernel beside them
 // ---- ops.cu
 void   launch_layernorm(const float * x, int64_t x_stride, const float * g, const float * b, float * y, int64_t y_stride,

@@ -26,17 +26,12 @@ struct XS {                 // activation row in shared memory
     const int8_t * q; const float * d; const float * s; const int16_t * bs;
 };
 
-__device__ __forceinline__ int dot16_u(const uint32_t w0, const uint32_t w1, const uint32_t w2, const uint32_t w3, const uint4 x) {
-    int s = dp4a_us(w0, (int) x.x, 0); s = dp4a_us(w1, (int) x.y, s); s = dp4a_us(w2, (int) x.z, s); return dp4a_us(w3, (int) x.w, s);
-}
 __device__ __forceinline__ uint4 lds16(const int8_t * p) { return *reinterpret_cast<const uint4 *>(p); }
 
 template <int TYPE> struct MV;
 
 // ---------------------------------------------------------------- Q4_K  (k_quants.c:1999-2055)
 // sum_j sc_j * (q4 . q8)_j and sum_j min_j * bsums_j as two dp2a over the expanded scale plane {sc0, sc1, m0, m1}
-__device__ __forceinline__ int dp2a_lo_us(int pair16, uint32_t bytes, int c) { int d; asm("dp2a.lo.s32.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(pair16), "r"(bytes), "r"(c)); return d; }
-__device__ __forceinline__ int dp2a_hi_us(int pair16, uint32_t bytes, int c) { int d; asm("dp2a.hi.s32.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(pair16), "r"(bytes), "r"(c)); return d; }
 __device__ __forceinline__ int pack16(int lo, int hi) { return (lo & 0xffff) | (hi << 16); }
 
 template <> struct MV<T_Q4_K> {
@@ -63,9 +58,9 @@ template <> struct MV<T_Q4_K> {
     __device__ static float dot(const Regs & r, int b, int pc, const XS & x) {
         const int e0 = b * 256 + 64 * (pc >> 1) + 16 * (pc & 1);          // low nibbles: e0.., high nibbles: e0+32..
         const uint4 xl = lds16(x.q + e0), xh = lds16(x.q + e0 + 32);
-        const int il = dot16_u(r.q.x & 0x0F0F0F0F, r.q.y & 0x0F0F0F0F, r.q.z & 0x0F0F0F0F, r.q.w & 0x0F0F0F0F, xl);
+        const int il = dot16(r.q.x & 0x0F0F0F0F, r.q.y & 0x0F0F0F0F, r.q.z & 0x0F0F0F0F, r.q.w & 0x0F0F0F0F, xl);
         // high nibbles stay in place (x16): the dot is an exact multiple of 16
-        const int ih = dot16_u(r.q.x & 0xF0F0F0F0, r.q.y & 0xF0F0F0F0, r.q.z & 0xF0F0F0F0, r.q.w & 0xF0F0F0F0, xh) >> 4;
+        const int ih = dot16(r.q.x & 0xF0F0F0F0, r.q.y & 0xF0F0F0F0, r.q.z & 0xF0F0F0F0, r.q.w & 0xF0F0F0F0, xh) >> 4;
         return finish(il, ih, r.sm, r.dd, b, pc, x);
     }
 };
@@ -92,8 +87,8 @@ template <> struct MV<T_Q5_K> {
         const int s0 = 2 * p, s1 = 2 * p + 1;
 #define LO5(w, hw) (((w) & 0x0F0F0F0F) | ((((hw) >> s0) & 0x01010101) << 4))
 #define HI5(w, hw) ((((w) >> 4) & 0x0F0F0F0F) | ((((hw) >> s1) & 0x01010101) << 4))
-        const int il = dot16_u(LO5(r.q.x, r.qh.x), LO5(r.q.y, r.qh.y), LO5(r.q.z, r.qh.z), LO5(r.q.w, r.qh.w), xl);
-        const int ih = dot16_u(HI5(r.q.x, r.qh.x), HI5(r.q.y, r.qh.y), HI5(r.q.z, r.qh.z), HI5(r.q.w, r.qh.w), xh);
+        const int il = dot16(LO5(r.q.x, r.qh.x), LO5(r.q.y, r.qh.y), LO5(r.q.z, r.qh.z), LO5(r.q.w, r.qh.w), xl);
+        const int ih = dot16(HI5(r.q.x, r.qh.x), HI5(r.q.y, r.qh.y), HI5(r.q.z, r.qh.z), HI5(r.q.w, r.qh.w), xh);
 #undef LO5
 #undef HI5
         // 5-bit codes: |il| can reach 16*31*127 > int16, so the scale products are plain 32-bit multiplies here
@@ -127,8 +122,8 @@ template <> struct MV<T_Q6_K> {
         const uint4 xl = lds16(x.q + b * 256 + el), xh = lds16(x.q + b * 256 + el + 64);
 #define LO6(w, hw) (((w) & 0x0F0F0F0F) | ((((hw) >> ls) & 0x03030303) << 4))
 #define HI6(w, hw) ((((w) >> 4) & 0x0F0F0F0F) | ((((hw) >> hs) & 0x03030303) << 4))
-        int il = dot16_u(LO6(r.ql.x, r.qh.x), LO6(r.ql.y, r.qh.y), LO6(r.ql.z, r.qh.z), LO6(r.ql.w, r.qh.w), xl);
-        int ih = dot16_u(HI6(r.ql.x, r.qh.x), HI6(r.ql.y, r.qh.y), HI6(r.ql.z, r.qh.z), HI6(r.ql.w, r.qh.w), xh);
+        int il = dot16(LO6(r.ql.x, r.qh.x), LO6(r.ql.y, r.qh.y), LO6(r.ql.z, r.qh.z), LO6(r.ql.w, r.qh.w), xl);
+        int ih = dot16(HI6(r.ql.x, r.qh.x), HI6(r.ql.y, r.qh.y), HI6(r.ql.z, r.qh.z), HI6(r.ql.w, r.qh.w), xh);
 #undef LO6
 #undef HI6
         il -= 32 * x.bs[b * 16 + (el >> 4)];                             // codes are stored +32
@@ -163,7 +158,7 @@ template <> struct MV<T_Q3_K> {
             const uint4 xv = lds16(x.q + b * 256 + el);
             const int hb = 4 * n + quad;
 #define C3(w, hw) ((((w) >> (2 * quad)) & 0x03030303) | ((((hw) >> hb) & 0x01010101) << 2))
-            int i = dot16_u(C3(r.q.x, r.hm.x), C3(r.q.y, r.hm.y), C3(r.q.z, r.hm.z), C3(r.q.w, r.hm.w), xv);
+            int i = dot16(C3(r.q.x, r.hm.x), C3(r.q.y, r.hm.y), C3(r.q.z, r.hm.z), C3(r.q.w, r.hm.w), xv);
 #undef C3
             i -= 4 * x.bs[b * 16 + (el >> 4)];                          // code = (q2 | hbit<<2) - 4
             isum += (int) (int8_t) (r.sc >> (8 * quad)) * i;
@@ -195,7 +190,7 @@ template <> struct MV<T_Q2_K> {
             const int el = 128 * n + 32 * quad + 16 * c;
             const uint4 xv = lds16(x.q + b * 256 + el);
 #define C2(w) (((w) >> (2 * quad)) & 0x03030303)
-            const int i = dot16_u(C2(r.q.x), C2(r.q.y), C2(r.q.z), C2(r.q.w), xv);
+            const int i = dot16(C2(r.q.x), C2(r.q.y), C2(r.q.z), C2(r.q.w), xv);
 #undef C2
             const int s = sc[el >> 4];
             isum += (s & 0xF) * i;
@@ -223,8 +218,8 @@ template <> struct MV<T_Q4_0> {
     }
     __device__ static float dot(const Regs & r, int b, int, const XS & x) {
         const uint4 xl = lds16(x.q + b * 32), xh = lds16(x.q + b * 32 + 16);
-        int s = dot16_u(r.q.x & 0x0F0F0F0F, r.q.y & 0x0F0F0F0F, r.q.z & 0x0F0F0F0F, r.q.w & 0x0F0F0F0F, xl);
-        s += dot16_u((r.q.x >> 4) & 0x0F0F0F0F, (r.q.y >> 4) & 0x0F0F0F0F, (r.q.z >> 4) & 0x0F0F0F0F, (r.q.w >> 4) & 0x0F0F0F0F, xh);
+        int s = dot16(r.q.x & 0x0F0F0F0F, r.q.y & 0x0F0F0F0F, r.q.z & 0x0F0F0F0F, r.q.w & 0x0F0F0F0F, xl);
+        s += dot16((r.q.x >> 4) & 0x0F0F0F0F, (r.q.y >> 4) & 0x0F0F0F0F, (r.q.z >> 4) & 0x0F0F0F0F, (r.q.w >> 4) & 0x0F0F0F0F, xh);
         s -= 8 * x.bs[b];
         return ((float) s * f16_bits_to_f32((uint16_t) r.d)) * x.d[b];
     }
@@ -243,8 +238,8 @@ template <> struct MV<T_Q4_1> {
     }
     __device__ static float dot(const Regs & r, int b, int, const XS & x) {
         const uint4 xl = lds16(x.q + b * 32), xh = lds16(x.q + b * 32 + 16);
-        int s = dot16_u(r.q.x & 0x0F0F0F0F, r.q.y & 0x0F0F0F0F, r.q.z & 0x0F0F0F0F, r.q.w & 0x0F0F0F0F, xl);
-        s += dot16_u((r.q.x >> 4) & 0x0F0F0F0F, (r.q.y >> 4) & 0x0F0F0F0F, (r.q.z >> 4) & 0x0F0F0F0F, (r.q.w >> 4) & 0x0F0F0F0F, xh);
+        int s = dot16(r.q.x & 0x0F0F0F0F, r.q.y & 0x0F0F0F0F, r.q.z & 0x0F0F0F0F, r.q.w & 0x0F0F0F0F, xl);
+        s += dot16((r.q.x >> 4) & 0x0F0F0F0F, (r.q.y >> 4) & 0x0F0F0F0F, (r.q.z >> 4) & 0x0F0F0F0F, (r.q.w >> 4) & 0x0F0F0F0F, xh);
         return (f16_bits_to_f32((uint16_t) (r.dm & 0xffff)) * x.d[b]) * (float) s + f16_bits_to_f32((uint16_t) (r.dm >> 16)) * x.s[b];
     }
 };
@@ -263,10 +258,10 @@ template <> struct MV<T_Q5_0> {
     }
     __device__ static int idot(const uint4 q, uint32_t qh, int b, const XS & x) {
         const uint4 xl = lds16(x.q + b * 32), xh = lds16(x.q + b * 32 + 16);
-        int s = dot16_u((q.x & 0x0F0F0F0F) | (spread4(qh) << 4), (q.y & 0x0F0F0F0F) | (spread4(qh >> 4) << 4),
-                        (q.z & 0x0F0F0F0F) | (spread4(qh >> 8) << 4), (q.w & 0x0F0F0F0F) | (spread4(qh >> 12) << 4), xl);
-        s += dot16_u(((q.x >> 4) & 0x0F0F0F0F) | (spread4(qh >> 16) << 4), ((q.y >> 4) & 0x0F0F0F0F) | (spread4(qh >> 20) << 4),
-                     ((q.z >> 4) & 0x0F0F0F0F) | (spread4(qh >> 24) << 4), ((q.w >> 4) & 0x0F0F0F0F) | (spread4(qh >> 28) << 4), xh);
+        int s = dot16((q.x & 0x0F0F0F0F) | (spread4(qh) << 4), (q.y & 0x0F0F0F0F) | (spread4(qh >> 4) << 4),
+                      (q.z & 0x0F0F0F0F) | (spread4(qh >> 8) << 4), (q.w & 0x0F0F0F0F) | (spread4(qh >> 12) << 4), xl);
+        s += dot16(((q.x >> 4) & 0x0F0F0F0F) | (spread4(qh >> 16) << 4), ((q.y >> 4) & 0x0F0F0F0F) | (spread4(qh >> 20) << 4),
+                   ((q.z >> 4) & 0x0F0F0F0F) | (spread4(qh >> 24) << 4), ((q.w >> 4) & 0x0F0F0F0F) | (spread4(qh >> 28) << 4), xh);
         return s;
     }
     __device__ static float dot(const Regs & r, int b, int, const XS & x) {
@@ -311,13 +306,6 @@ template <> struct MV<T_Q8_0> {
         return (float) s * (f16_bits_to_f32((uint16_t) r.d) * x.d[b]);
     }
 };
-
-// fp16-LUT-equivalent GELU (ggml.c:3461-3484): f16 in, fp32 formula, f16 out
-__device__ __forceinline__ float gelu_f16lut(float v) {
-    const float f = __half2float(__float2half_rn(v));
-    const float g = 0.5f * f * (1.0f + tanhf(0.79788456080286535587989211986876f * f * (1.0f + 0.044715f * f * f)));
-    return __half2float(__float2half_rn(g));
-}
 
 // ------------------------------------------------------------------------------------------------ the kernel
 // Work unit = CH consecutive blocks of one weight row (about 4-5 KB over all planes).  Every warp owns a ring of
@@ -437,12 +425,6 @@ __global__ void __launch_bounds__(MMV_THREADS, 1) mmv_kernel(const WPlanes W, co
     }
 }
 
-static int g_num_sms = 0;
-static int num_sms() {
-    if (!g_num_sms) { int dev; B200_CUDA_CHECK(cudaGetDevice(&dev)); B200_CUDA_CHECK(cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev)); }
-    return g_num_sms;
-}
-
 template <int TYPE>
 static void launch_typed(const WPlanes & W, const ActQ & A, float * y, int64_t y_stride, MmvEpilogue epi, cudaStream_t stream) {
     using G = UnitGeom<TYPE>;
@@ -464,8 +446,6 @@ static void launch_typed(const WPlanes & W, const ActQ & A, float * y, int64_t y
     mmv_kernel<TYPE><<<grid, MMV_THREADS, smem, stream>>>(W, A, y, y_stride, epi, S);
     B200_CUDA_CHECK(cudaGetLastError());
 }
-
-bool launch_mmv_fast(const WPlanes & W, const ActQ & A, float * y, int64_t y_stride, MmvEpilogue e, cudaStream_t stream);   // mmv_fast.cu
 
 void launch_mmv(const WPlanes & W, const ActQ & A, float * y, int64_t y_stride, MmvEpilogue epi, cudaStream_t stream) {
     B200_ASSERT(A.K == W.K && A.type == act_type_for(W.type));

@@ -326,13 +326,8 @@ void launch_layernorm_q(float * x, int64_t x_stride, const float * ra, const flo
 }
 
 // ---------------------------------------------------------------------------------------------- elementwise
-__device__ __forceinline__ float gelu_ref(float v) {      // table_gelu_f16[f16(v)] (ggml.c:3476-3484, table 4281-4290)
-    const float f = __half2float(__float2half_rn(v));
-    const float gl = 0.5f * f * (1.0f + tanhf(0.79788456080286535587989211986876f * f * (1.0f + 0.044715f * f * f)));
-    return __half2float(__float2half_rn(gl));
-}
 __global__ void gelu_kernel(const float * __restrict__ x, float * __restrict__ y, int64_t n) {
-    for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x * blockDim.x) y[i] = gelu_ref(x[i]);
+    for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x * blockDim.x) y[i] = gelu_f16lut(x[i]);
 }
 __global__ void add_kernel(const float * __restrict__ a, const float * __restrict__ b, float * __restrict__ y, int64_t n) {
     for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x * blockDim.x) y[i] = __fadd_rn(a[i], b[i]);

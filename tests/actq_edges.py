@@ -6,8 +6,8 @@ Random fp32 rows never reach the rules that matter, so every block here is built
 that it really exercises it (a tie that is not on the block maximum tests nothing):
 
   E1  sign tie on the block maximum: +a before -a and -a before +a, inside one lane's 8 values, across lanes at every xor distance
-      of the block reductions (1, 2 for 32-blocks; 1, 2, 4, 8, 16 for 256-blocks), across the two 16-value segments of the Q4_K
-      mat-vec prologue (FX<T_Q4_K>::quant_x), with the earlier element in the lower and in the higher lane.  For Q8_K the first
+      of the block reductions (1, 2 for 32-blocks; 1, 2, 4, 8, 16 for 256-blocks), across the two 16-value segments one Q4_K
+      mat-vec piece multiplies (32 values apart), with the earlier element in the lower and in the higher lane.  For Q8_K the first
       element of largest magnitude sets the sign of d and which element is clamped; Q8_0 / Q8_1 only read the magnitude.
   E2  repeated equal magnitudes of the same sign on the fp16 grid (what fp16-grid producers such as GELU hand over).
   E3  products v * id (Q8_0 / Q8_1) or iscale * v (Q8_K) that are exactly k + 1/2, both parities and both signs, where

@@ -70,7 +70,7 @@ def test_oracle_quantiser_is_the_reference_on_edge_rows(wt):
 
 # the producers of the activation codes (and the fp16 GEMM operand) and the activation types each one supports
 PRODUCERS = {"standalone": ae.ATYPES, "ln_cluster": ae.ATYPES, "ln_reg1": ae.ATYPES, "ln_reg2": ae.ATYPES, "ln_smem": ae.ATYPES,
-             "attn split": ae.ATYPES, "attn long": ae.ATYPES, "chain": (po.Q8_K, po.Q8_0), "fused": (po.Q8_K, po.Q8_0),
+             "attn split": ae.ATYPES, "attn long": ae.ATYPES, "chain": (po.Q8_K, po.Q8_0),
              "plane standalone": ae.ATYPES, "plane ln_reg1": ae.ATYPES, "plane ln_reg2": ae.ATYPES, "plane ln_smem": ae.ATYPES}
 
 
@@ -85,8 +85,7 @@ def test_parametrisation_reaches_every_producer_and_family():
                for p, ats in PRODUCERS.items() for at in ats if need(p, at) - got.get((p, at), set())]
     assert not missing, missing
     assert {k[0] for k in got} == set(PRODUCERS)
-    # the cases behind the keys: each LayerNorm kernel and both attention tiers with every type, both fused prologue types
+    # the cases behind the keys: each LayerNorm kernel and both attention tiers with every type
     assert set(G.LN_KERNEL.values()) == {"ln_cluster", "ln_reg1", "ln_reg2", "ln_smem"}
     assert {po.VEC_DOT_TYPE[wt] for _, _, wt in G.ATTN} == set(ae.ATYPES)
     assert any(G_ % 4 == 0 for G_, _, wt in G.ATTN if wt == po.Q4_K)            # Q8_K folds into the attention only when G % 4 == 0
-    assert {po.VEC_DOT_TYPE[wt] for wt, _ in G.FUSED} == {po.Q8_K, po.Q8_0}

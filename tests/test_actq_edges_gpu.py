@@ -6,8 +6,6 @@ How each producer is fed a chosen row:
   standalone      quantize_act on the rows directly (N = 1, 9, 40, x_stride > K)
   LayerNorm       gamma = 0, beta = the row: norm(x) * 0 is +-0 and +-0 + beta = beta, so the row to quantise is beta exactly
                   (every variant: cluster, register CH = 1 / 2, shared memory; single and dual; with and without the residual adds)
-  fused mat-vec   modes 1 (the row) and 2 (gamma = 0, beta = the row) with selector weights: M = K rows, row m is +1 at k = m and
-                  exact zeros elsewhere, so y[m] = float32(code[m]) * d[block of m] exactly and the prologue's codes are observable
   chain           an input whose quantisation is exact (Q8_K blocks of maximum -128 * 2^a, Q8_0 blocks of maximum 127 * 2^a) and
                   selector weights with power-of-two scales make y equal the designed row; a_out is then checked against it
   attention       n_past = 0: one key of weight exactly 1.  The split-KV kernel's output is then the new V row (asserted, by value:
@@ -28,7 +26,6 @@ STANDALONE_N = [1, 9, 40]
 LN_VARIANTS = {"cluster": (8192, 1, None), "reg1": (8192, 3, None), "reg1_rows1": (8192, 1, "B200_LN_NOCLUSTER"),
                "reg2": (14848, 2, None), "smem": (18432, 2, None), "smem_env": (4096, 3, "B200_LN_SMEM")}
 LN_KERNEL = {"cluster": "ln_cluster", "reg1": "ln_reg1", "reg1_rows1": "ln_reg1", "reg2": "ln_reg2", "smem": "ln_smem", "smem_env": "ln_smem"}
-FUSED = [(po.Q4_K, 8192), (po.Q4_0, 4544)]
 CHAIN = {po.Q4_K: ((-100, 0, 95), 12288), po.Q4_0: ((-12, 0, 12), 1024)}      # input block exponents, output length M
 ATTN = [(16, 8, po.Q4_K), (71, 2, po.Q4_0), (8, 8, po.Q4_1)]                   # (G, n_head_kv, weight type)
 ATTN_TIERS = ["split", "long"]
@@ -42,10 +39,6 @@ def standalone_rows(at):
 
 def ln_rows(at, variant):
     return ae.edge_rows(at, LN_VARIANTS[variant][0])
-
-
-def fused_rows(wt, K):
-    return ae.edge_rows(po.VEC_DOT_TYPE[wt], K)
 
 
 def attn_rows(G, hkv, wt, tier):
@@ -108,8 +101,6 @@ def reached():
             add((LN_KERNEL[v], at), ln_rows(at, v)[1])
             if LN_VARIANTS[v][1] > 1:
                 add(("plane " + LN_KERNEL[v], at), ln_rows(at, v)[1])
-    for wt, K in FUSED:
-        add(("fused", po.VEC_DOT_TYPE[wt]), fused_rows(wt, K)[1])
     for wt in CHAIN:
         add(("chain", po.VEC_DOT_TYPE[wt]), chain_rows(wt)[1])
     for G, hkv, wt in ATTN:
@@ -240,7 +231,7 @@ def test_layernorm_quantiser_real_gamma_beta(gpu, orc, monkeypatch, at, variant)
         _check_plane(gpu, at, A, q, d, "%s real" % variant)
 
 
-# ------------------------------------------------------------------------------------------------ fused mat-vec prologues
+# ------------------------------------------------------------------------------------------------ chain hand-over
 def selector_blocks(wt, K, src, dexp=None):
     """raw Q4_K / Q4_0 blocks of M = len(src) rows: row m is +1 (times 2^dexp[m]) at k = src[m] and exactly 0 elsewhere.
     Q4_K: d = 2^dexp, dmin = 0, every sub-block scale 1 and min 0, code 1 at k, 0 elsewhere; blocks not holding k have d = 0.
@@ -271,32 +262,6 @@ def selector_blocks(wt, K, src, dexp=None):
     return b.reshape(M, -1)
 
 
-@gpu_mark
-@pytest.mark.parametrize("mode", [1, 2])
-@pytest.mark.parametrize("wt,K", FUSED)
-def test_fused_prologue_codes(gpu, orc, wt, K, mode):
-    at = po.VEC_DOT_TYPE[wt]
-    W = gpu.Weight(wt, K, K, selector_blocks(wt, K, np.arange(K)))
-    rows, labels = fused_rows(wt, K)
-    rng = np.random.default_rng(K)
-    yd = gpu.DevBuf(K * 4)
-    zero = gpu.DevBuf(src=np.zeros(K, F32))
-    for r in range(rows.shape[0]):
-        if mode == 1:
-            xd = gpu.DevBuf(src=rows[r])
-            assert gpu.lib().b200_mul_mat_vec_fused(W.h, xd.ptr, None, None, None, None, None, yd.ptr, 0) == 1
-        else:
-            xd, bd = gpu.DevBuf(src=(rng.standard_normal(K) * 2 + 0.5).astype(F32)), gpu.DevBuf(src=rows[r])
-            assert gpu.lib().b200_mul_mat_vec_fused(W.h, xd.ptr, None, None, zero.ptr, bd.ptr, None, yd.ptr, 0) == 1
-        y = yd.download(F32, (K,))
-        q, d, _, _ = _want(orc, at, rows[r][None, :])
-        want = q[0].astype(F32) * np.repeat(d[0], ae.BLK[at])
-        bad = y != want                                  # value equality: a zero code gives +-0 depending on the sign of d
-        assert not bad.any(), ("mode %d row %d" % (mode, r), labels[r][np.flatnonzero(bad)[0] // ae.BLK[at]],
-                               int(np.flatnonzero(bad)[0]), float(y[bad][0]), float(want[bad][0]))
-
-
-# ------------------------------------------------------------------------------------------------ chain hand-over
 @gpu_mark
 @pytest.mark.parametrize("wt", list(CHAIN))
 def test_chain_handover_on_edge_rows(gpu, orc, wt):

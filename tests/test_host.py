@@ -199,7 +199,7 @@ def test_launch_list_tool_pivots_an_ncu_csv(tmp_path):
     for step in range(3):                                   # the third step is cut short by the capture limit
         launch("dequant_rows_kernel(WPlanes, const int *, int, float *, long)", 5000, 1e4)
         for i in range(4 if step < 2 else 2):
-            launch("void mmv_fast_kernel<12, 256, 1, 8, 0>(WPlanes, FastX, float *, long, Epi)", 20000, 80e6)
+            launch("void mmv_fast_kernel<12, 256, 1, 8>(WPlanes, ActQ, float *, long, Epi)", 20000, 80e6)
         launch("attn_dec_scores_kernel(AttnDecArgs)", 6000, 1e5)
     raw, out, tr = tmp_path / "raw.csv", tmp_path / "out.csv", tmp_path / "traffic.json"
     with open(raw, "w", newline="") as f:

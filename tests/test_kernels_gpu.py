@@ -287,50 +287,6 @@ def test_tensor_core_gemm_operand_is_the_exact_fp16_weight(gpu, orc, t, N):
         assert np.array_equal(got, want[:, cols].T), (t, N, off)
 
 
-@pytest.mark.parametrize("t,K,M", [(po.Q4_K, 8192, 700), (po.Q4_K, 14848, 300), (po.Q4_0, 4544, 333), (po.Q4_K, 256, 64)])
-def test_fused_layernorm_quantize_matvec(gpu, orc, t, K, M):
-    """residual adds + LayerNorm + Q8 quantisation in the mat-vec prologue == the separate CPU ops, and the updated
-    residual row is written out bit-exactly"""
-    rng = np.random.default_rng(K + M)
-    wq = _weights(orc, t, M, K, seed=5)
-    x, ra, rb = (rng.standard_normal(K).astype(np.float32) for _ in range(3))
-    g = (1 + 0.1 * rng.standard_normal(K)).astype(np.float32)
-    b = (0.01 * rng.standard_normal(K)).astype(np.float32)
-    W = gpu.Weight(t, K, M, wq)
-    xd, rad, rbd, gd, bd = (gpu.DevBuf(src=a) for a in (x, ra, rb, g, b))
-    xo, yd = gpu.DevBuf(K * 4), gpu.DevBuf(M * 4)
-    assert gpu.lib().b200_mul_mat_vec_fused(W.h, xd.ptr, rad.ptr, rbd.ptr, gd.ptr, bd.ptr, xo.ptr, yd.ptr, 0) == 1
-    resid = (ra + rb) + x
-    assert np.array_equal(xo.download(np.float32, (K,)), resid)
-    ln = orc.layernorm(resid[None, :], g, b)
-    want = orc.mul_mat(t, wq, K, M, ln)[0]
-    got = yd.download(np.float32, (M,))
-    wd = np.abs(orc.dequantize(t, wq, K))
-    # LayerNorm's double sums are reduced in a different order: allow one activation code to move (1/127 of a block maximum)
-    budget = 2e-5 * (wd @ np.abs(ln[0])) + np.abs(wd).max(1) * np.abs(ln).max() / 127 + 1e-6
-    assert np.all(np.abs(got - want) <= budget), float(np.abs(got - want).max())
-    assert np.median(np.abs(got - want)) <= 1e-5 * np.abs(want).max()
-    # plain quantise-in-prologue (ffn_down / wo inputs), with the GELU epilogue
-    assert gpu.lib().b200_mul_mat_vec_fused(W.h, xd.ptr, None, None, None, None, None, yd.ptr, 0) == 1
-    want = orc.mul_mat(t, wq, K, M, x[None, :])[0]
-    got = yd.download(np.float32, (M,))
-    assert np.all(np.abs(got - want) <= 2e-5 * (wd @ np.abs(x)) + 1e-6)
-
-
-def test_fused_matvec_large_k(gpu, orc):
-    """K = 32768 (ffn_down): four pieces per thread, quantise-in-prologue"""
-    t, K, M = po.Q4_K, 32768, 130
-    rng = np.random.default_rng(1)
-    wq = _weights(orc, t, M, K, seed=6)
-    x = rng.standard_normal(K).astype(np.float32)
-    W = gpu.Weight(t, K, M, wq)
-    xd, yd = gpu.DevBuf(src=x), gpu.DevBuf(M * 4)
-    assert gpu.lib().b200_mul_mat_vec_fused(W.h, xd.ptr, None, None, None, None, None, yd.ptr, 0) == 1
-    want = orc.mul_mat(t, wq, K, M, x[None, :])[0]
-    wd = np.abs(orc.dequantize(t, wq, K))
-    assert np.all(np.abs(yd.download(np.float32, (M,)) - want) <= 2e-5 * (wd @ np.abs(x)) + 1e-6)
-
-
 @pytest.mark.parametrize("t,K,M", [(po.Q4_K, 8192, 32768), (po.Q4_K, 512, 768), (po.Q4_0, 4544, 18176)])
 def test_matvec_chain_quantises_output_for_next_matmul(gpu, orc, t, K, M):
     """ffn_up -> ffn_down hand-over: the mat-vec's own CTAs quantise the (GELU'd) output row, 256 values at a time, as

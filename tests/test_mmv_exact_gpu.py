@@ -27,7 +27,8 @@ FAST = [(L4K, 2048, 301, 1, None), (L4K, 8192, 9216, 1, None), (L4K, 4352, 37, 2
         (L40, 65536, 37, 1, None), (L40, 65568, 5, 1, None),
         (L3K, 8192, 9216, 1, None), (L3K, 14848, 37, 2, None), (L3K, 32768, 37, 8, None), (L3K, 59392, 37, 1, None),
         (L3K, 65792, 5, 1, None),
-        (L4K, 14848, 37, 1, "B200_NO_NT256J2"), (L4K, 4352, 5, 1, "B200_NO_NT160"), (L40, 4544, 37, 1, "B200_NO_NT160"),
+        (L4K, 14848, 37, 1, "B200_NO_NT256J2"), (L40, 14848, 37, 1, "B200_NO_NT256J2"), (L4K, 4352, 5, 1, "B200_NO_NT160"),
+        (L40, 4544, 37, 1, "B200_NO_NT160"),
         (L4K, 18432, 37, 1, "B200_NO_NT192"), (L40, 18176, 37, 2, "B200_NO_NT192")]
 # the generic ring kernel (mmv.cu): K with one, two and more work units per row and a ragged last unit, for every type; the
 # types the tuned kernel covers go there through B200_MMV_GENERIC
@@ -37,14 +38,14 @@ GENERIC += [(po.Q6_K, 8192, 9216, 1, None), (po.Q5_K, 32768, 8192, 1, None), (po
             (po.Q8_0, 18176, 4544, 1, None)]
 
 
-def _shape(t, K, mode, env):
+def _shape(t, K, env):
     os.environ.pop("B200_MMV_GENERIC", None)
     old = {k: os.environ.pop(k, None) for k in ENV_SWITCHES}
     try:
         if env:
             os.environ[env] = "1"
         import ggllm_cpp_b200.binding as b
-        return None if env == "B200_MMV_GENERIC" else b.mmv_launch_shape(t, K, mode)
+        return None if env == "B200_MMV_GENERIC" else b.mmv_launch_shape(t, K)
     finally:
         if env:
             os.environ.pop(env, None)
@@ -118,7 +119,7 @@ def _cid(c):
 @pytest.mark.parametrize("case", FAST + GENERIC, ids=_cid)
 def test_mat_vec_within_exact_bound(gpu, orc, case):
     t, K, M, N, env = case
-    shape = _shape(t, K, 0, env)
+    shape = _shape(t, K, env)
     wq, x, W, A, act = _setup(gpu, orc, t, K, M, N, seed=K + M + N)
     yd = gpu.DevBuf(N * M * 4)
     with _env(env):
@@ -134,7 +135,7 @@ EPI = [(L4K, 8192, 301, None), (L40, 14848, 301, None), (po.Q5_K, 18432, 301, No
 @pytest.mark.parametrize("case", EPI, ids=lambda c: "%s-K%d%s" % (po.TYPE_NAMES[c[0]], c[1], "-generic" if c[3] else ""))
 def test_mat_vec_epilogues_within_exact_bound(gpu, orc, case, epi):
     t, K, M, env = case
-    shape = _shape(t, K, 0, env)
+    shape = _shape(t, K, env)
     wq, x, W, A, act = _setup(gpu, orc, t, K, M, 1, seed=K + epi)
     rng = np.random.default_rng(epi)
     r1, r2 = (rng.standard_normal((1, M)) * 64).astype(np.float32), (rng.standard_normal((1, M)) * 64).astype(np.float32)
@@ -145,21 +146,6 @@ def test_mat_vec_epilogues_within_exact_bound(gpu, orc, case, epi):
 
 
 @gpu_mark
-@pytest.mark.parametrize("t,K", [(L4K, 14848), (L40, 14848), (L40, 18176)])
-def test_fused_quantising_prologue_within_exact_bound(gpu, orc, t, K):
-    """mode 1 (b200_mul_mat_vec_fused without LayerNorm): the prologue quantises the fp32 row exactly as quantize_act does, so the
-    restatement from the oracle's codes applies unchanged"""
-    M = 301
-    rng = np.random.default_rng(K)
-    wq = mx.swept_weights(t, M, K, rng)
-    x = mx.swept_acts(t, 1, K, rng)
-    W, xd, yd = gpu.Weight(t, K, M, wq), gpu.DevBuf(src=x), gpu.DevBuf(M * 4)
-    assert gpu.lib().b200_mul_mat_vec_fused(W.h, xd.ptr, None, None, None, None, None, yd.ptr, 0) == 1
-    q, d, s, _ = mx.act_from_blocks(t, orc.quantize_act(t, x), K)
-    _check(t, K, wq, yd.download(np.float32, (1, M)), (q, d, s), _shape(t, K, 1, None))
-
-
-@gpu_mark
 def test_chain_at_falcon_180b_width(gpu, orc):
     """b200_mul_mat_vec_q_chain at Falcon-180B's ffn_up shape (K = 14848, M = 59392): the output row within the bound (its
     quantised hand-over is checked bit for bit against quantize_act in test_kernels_gpu.py)"""
@@ -167,7 +153,7 @@ def test_chain_at_falcon_180b_width(gpu, orc):
     wq, x, W, A, act = _setup(gpu, orc, t, K, M, 1, seed=180)
     A_out, yd = gpu.ActQ(t, M, 1), gpu.DevBuf(M * 4)
     assert gpu.lib().b200_mul_mat_vec_q_chain(W.h, A.h, yd.ptr, 0, A_out.h) == 1
-    _check(t, K, wq, yd.download(np.float32, (1, M)), act, _shape(t, K, 0, None))
+    _check(t, K, wq, yd.download(np.float32, (1, M)), act, _shape(t, K, None))
 
 
 @gpu_mark
@@ -187,22 +173,20 @@ def test_float_weight_mat_vec_within_exact_bound(gpu, orc, t, K, M):
 
 
 def test_parametrisation_reaches_every_launch_shape():
-    """every (NT, J, D) the launch-shape choice can return for Q4_K, Q4_0 and Q3_K, in any mode and under any of its switches, is
-    run by test_mat_vec_within_exact_bound or the prologue test; and K past 64 Ki goes to the generic kernel"""
+    """every (NT, J, D) the launch-shape choice can return for Q4_K, Q4_0 and Q3_K, under any of its switches, is run by
+    test_mat_vec_within_exact_bound; and K past 64 Ki goes to the generic kernel"""
     import ggllm_cpp_b200.binding as b
     if not os.path.exists(b.LIB_PATH):
         b.build()
     possible = set()
     for t in (L4K, L40, L3K):
         for env in (None,) + ENV_SWITCHES:
-            for mode in ((0,) if t == L3K else (0, 1, 2)):
-                for K in range(256, 70000, 256):
-                    s = _shape(t, K, mode, env)
-                    if s is not None:
-                        possible.add((t, s))
-        assert _shape(t, 65536 + 256, 0, None) is None
-    reached = {(c[0], _shape(c[0], c[1], 0, c[4])) for c in FAST}
-    reached |= {(t, _shape(t, K, 1, None)) for t, K in ((L4K, 14848), (L40, 14848), (L40, 18176))}
+            for K in range(256, 70000, 256):
+                s = _shape(t, K, env)
+                if s is not None:
+                    possible.add((t, s))
+        assert _shape(t, 65536 + 256, None) is None
+    reached = {(c[0], _shape(c[0], c[1], c[4])) for c in FAST}
     missing = possible - reached
     assert not missing, sorted(missing)
     assert len(possible) >= 15
