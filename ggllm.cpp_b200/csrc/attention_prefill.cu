@@ -1,4 +1,5 @@
-// attention_prefill.cu -- causal grouped-query attention for a batch of N > 1 new tokens (prompt processing).
+// attention_prefill.cu -- causal grouped-query attention for a batch of N > 1 new tokens (prompt processing) where attention_ws.cu
+// does not apply (N <= 8, no fp16 shadow, head_dim != 64).
 //
 // Same arithmetic contract as attention.cu (libfalcon.cpp:2285-2366, ggml.c:12389-12458): fp32 scores, softmax with the
 // row's GLOBAL maximum subtracted before an fp16-LUT exp, the sum accumulated in double, probabilities scaled by
@@ -14,8 +15,6 @@
 
 #define PT 64          // tile: 64 rows x 64 keys (scores) / 64 rows x 64 dims (PV)
 #define PTHREADS 256
-
-__device__ __forceinline__ float exp_lut(float v) { return __half2float(__float2half_rn(expf(__half2float(__float2half_rn(v))))); }
 
 struct PrefillArgs {
     const float * qkv; const float * kc; const float * vc; float * out; float * S; float * inv;
@@ -89,7 +88,7 @@ __global__ void __launch_bounds__(PTHREADS) prefill_scores_kernel(const PrefillA
             const int t = row / a.G, vis = a.n_past + t + 1;
             const float mx = smax[r];
             float * Sr = Sg + (size_t) row * a.s_stride;
-            for (int k = part; k < vis; k += 4) { const float e = exp_lut(__fsub_rn(Sr[k], mx)); Sr[k] = e; sum += (double) e; }
+            for (int k = part; k < vis; k += 4) { const float e = exp_f16lut(__fsub_rn(Sr[k], mx)); Sr[k] = e; sum += (double) e; }
         }
         sum += __shfl_xor_sync(0xffffffffu, sum, 1);
         sum += __shfl_xor_sync(0xffffffffu, sum, 2);

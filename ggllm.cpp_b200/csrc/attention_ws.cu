@@ -259,11 +259,13 @@ void launch_kv_shadow_refresh(const float * k_cache, const float * v_cache, __ha
     B200_CUDA_CHECK(cudaGetLastError());
 }
 
-// false: not covered (no shadow, head_dim != 64, small batch) -> the caller falls back to attention_prefill.cu
-bool launch_attention_ws(const float * qkv, float * out, int64_t out_stride, const AttnParams & p, cudaStream_t stream) {
-    if (!p.k16 || !p.vt16 || p.head_dim != D || p.n_past_dev != nullptr || getenv("B200_ATTN_SIMT")) return false;
-    if (p.n_tok <= b200_mmv_max_n() && !getenv("B200_ATTN_TC")) return false;     // small batches keep fp32 attention (reassociation-level parity)
-    if ((p.qkv_stride % 4) != 0 || (out_stride % 4) != 0) return false;
+// the shapes this kernel takes: an fp16 shadow, head_dim 64, a host n_past, more than b200_mmv_max_n() tokens (B200_ATTN_TC: also fewer)
+bool attention_ws_covers(const AttnParams & p) {
+    if (!p.k16 || !p.vt16 || p.head_dim != D || p.n_past_dev != nullptr || (p.qkv_stride % 4) != 0 || getenv("B200_ATTN_SIMT")) return false;
+    return p.n_tok > b200_mmv_max_n() || getenv("B200_ATTN_TC");     // small batches keep fp32 attention (reassociation-level parity)
+}
+void launch_attention_ws(const float * qkv, float * out, int64_t out_stride, const AttnParams & p, cudaStream_t stream) {
+    B200_ASSERT(out_stride % 4 == 0);
     WsArgs a;
     a.qkv = qkv; a.out = out;
     a.n_head_kv = p.n_head_kv; a.G = p.n_head / p.n_head_kv; a.n_tok = p.n_tok; a.n_past = p.n_past; a.T = p.n_past + p.n_tok;
@@ -294,5 +296,4 @@ bool launch_attention_ws(const float * qkv, float * out, int64_t out_stride, con
     dim3 grid((unsigned) ((a.rows + M - 1) / M), (unsigned) p.n_head_kv);
     attention_ws_kernel<<<grid, THREADS, SMEM_BYTES, stream>>>(kmap, vmap, a);
     B200_CUDA_CHECK(cudaGetLastError());
-    return true;
 }

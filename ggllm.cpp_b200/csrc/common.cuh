@@ -111,6 +111,21 @@ __device__ __forceinline__ float gelu_f16lut(float v) {
     const float g = 0.5f * f * (1.0f + tanhf(0.79788456080286535587989211986876f * f * (1.0f + 0.044715f * f * f)));
     return __half2float(__float2half_rn(g));
 }
+// table_exp_f16[f16(v)] (ggml.c:4281-4290), the softmax exponential of every attention kernel but the wgmma one
+__device__ __forceinline__ float exp_f16lut(float v) {
+    return __half2float(__float2half_rn(expf(__half2float(__float2half_rn(v)))));
+}
+
+// NeoX RoPE (ggml.c:12819-12983).  Pair i of a head at position p: theta = p * theta_scale^i built by repeated fp32 products, as the
+// CPU loop does, then (x0, x1) -> (x0 c - x1 s, x0 s + x1 c) with every product and sum rounded on its own.
+__device__ __forceinline__ float rope_theta(int p, int i, float theta_scale) {
+    float theta = (float) p;
+    for (int k = 0; k < i; k++) theta = __fmul_rn(theta, theta_scale);
+    return theta;
+}
+__device__ __forceinline__ float2 rope_rotate(float x0, float x1, float c, float s) {
+    return make_float2(__fsub_rn(__fmul_rn(x0, c), __fmul_rn(x1, s)), __fadd_rn(__fmul_rn(x0, s), __fmul_rn(x1, c)));
+}
 
 // ---- mbarrier + 1-D bulk (TMA) copy global -> shared: used to stage activation tiles ----
 __device__ __forceinline__ uint32_t smem_u32(const void * p) { return (uint32_t) __cvta_generic_to_shared(p); }

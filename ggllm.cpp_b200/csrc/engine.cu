@@ -75,8 +75,8 @@ struct b200_falcon {
     float * inp = nullptr, * qkv = nullptr, * att = nullptr, * ao = nullptr, * up = nullptr, * dn = nullptr, * logits = nullptr;
     void * actq_mem = nullptr; ActQ xa{}, xm{}, xatt{}, xup{}, xf{};
     __half * xh_a = nullptr, * xh_b = nullptr, * xh_m = nullptr;      // fp16 GEMM operands (d * q), written by the kernels that quantise: attention branch, MLP branch, MLP input
-    float * attn_scratch = nullptr;
-    float * attn_dec_scratch = nullptr;            // split-KV decode attention: counters + scores + partials (attention.cu)
+    float * attn_scratch = nullptr; size_t attn_scratch_bytes = 0;     // prompt attention (grown on demand)
+    float * attn_dec_scratch = nullptr;            // decode attention: zeroed before the decode graphs are captured
     int32_t * tokens_dev = nullptr; int * n_past_dev = nullptr;
     int32_t * tokens_h = nullptr; int * n_past_h = nullptr; float * logits_h = nullptr; size_t logits_h_floats = 0;
     cudaStream_t s_main = nullptr, s_mlp = nullptr;
@@ -594,26 +594,28 @@ static void eval_output(b200_falcon * f, int N, int logits_rows_from, bool fold_
 
 // AttnParams of local layer l for N new tokens.  graph_mode: n_past is read from the device scalar, and the tier the graph is captured
 // for (cur_tier) says whether the long-context kernels may be captured.
-static AttnParams attn_params(const b200_falcon * f, int l, int N, int n_past, bool graph_mode) {
+static AttnParams attn_params(const b200_falcon * f, int l, int N, int n_past, float theta_scale, bool graph_mode) {
     AttnParams ap = { f->H, f->HKV, f->D, N, n_past, graph_mode ? f->n_past_dev : nullptr, f->hp.n_ctx, (int64_t) f->QKV, nullptr };
     ap.long_ctx = graph_mode ? f->cur_tier : 0;
+    ap.rope_theta_scale = theta_scale;
     const KvLayer kv = kv_layer(f, l);
     ap.k16 = kv.k16; ap.vt16 = kv.vt16;
     return ap;
 }
-// RoPE + KV append of layer l's new rows (:2229-2281) unless the decode attention launch does them itself (ap.fuse_rope), then the
-// attention qkv -> att (:2285-2366).  A prompt with a host n_past takes the tensor-core kernel (no scratch); where that does not apply
-// (N <= 8, head_dim != 64) the CUDA-core kernels, which materialise the score matrix in a scratch buffer.
-static void enqueue_attention(b200_falcon * f, int l, const AttnParams & ap, float theta_scale, cudaStream_t st) {
+// RoPE + KV append of layer l's new rows (:2229-2281), then the attention qkv -> att (:2285-2366).  Prompts run eagerly, on s_main
+// like their attention: a scratch that has to grow waits for the previous user.
+static void enqueue_attention(b200_falcon * f, int l, const AttnParams & ap, cudaStream_t st) {
     const KvLayer kv = kv_layer(f, l);
-    if (!ap.fuse_rope) { launch_rope_kv_append(f->qkv, kv.k, kv.v, ap, theta_scale, st); f->launches++; }
-    if (ap.n_tok == 1 || ap.n_past_dev)
-        f->launches += launch_attention(f->qkv, kv.k, kv.v, f->att, f->E, ap, ap.n_tok == 1 ? f->attn_dec_scratch : nullptr, st);
-    else if (launch_attention_ws(f->qkv, f->att, f->E, ap, st)) f->launches++;
-    else {
-        if (!f->attn_scratch) B200_CUDA_CHECK(cudaMalloc(&f->attn_scratch, attention_prefill_scratch_bytes(f->H, f->hp.n_batch, f->hp.n_ctx)));
-        launch_attention_prefill(f->qkv, kv.k, kv.v, f->att, f->E, ap, f->attn_scratch, st); f->launches += 2;
+    float * scratch = f->attn_dec_scratch;
+    if (ap.n_tok > 1) {
+        const size_t need = attention_scratch_bytes(ap);
+        if (need > f->attn_scratch_bytes) {
+            B200_CUDA_CHECK(cudaStreamSynchronize(st)); B200_CUDA_CHECK(cudaFree(f->attn_scratch));
+            B200_CUDA_CHECK(cudaMalloc(&f->attn_scratch, need)); f->attn_scratch_bytes = need;
+        }
+        scratch = f->attn_scratch;
     }
+    f->launches += launch_attention(f->qkv, kv.k, kv.v, f->att, f->E, ap, scratch, st);
 }
 
 static bool fused_decode_ok(const b200_falcon * f) {
@@ -660,14 +662,10 @@ static void enqueue_decode_fused(b200_falcon * f, int n_past, float theta_scale,
         B200_CUDA_CHECK(cudaEventRecord(f->e_fork, sa));
         B200_CUDA_CHECK(cudaStreamWaitEvent(sb, f->e_fork, 0));
         if (!skip("attn")) {
-            AttnParams ap = attn_params(f, l, 1, n_past, graph_mode);
-            ap.fuse_rope = 1; ap.rope_theta_scale = theta_scale;
-            // wo's activation quantisation: done by the attention kernel's combine step when its blocks fit the head groups,
-            // else by a kernel of its own; either way off the critical path
-            const bool fold_q = f->attn_dec_scratch && f->D == 64 && !getenv("B200_ATTN_NOSPLIT") && !getenv("B200_ATTN_NOFOLD") && (xatt.type != T_Q8_K || (f->H / f->HKV) % 4 == 0);
-            if (fold_q) ap.qout = &xatt;
-            enqueue_attention(f, l, ap, theta_scale, sb);
-            if (!fold_q) { launch_quantize_act(f->att, E, xatt, sb); f->launches++; }
+            AttnParams ap = attn_params(f, l, 1, n_past, theta_scale, graph_mode);
+            ap.fuse_rope = 1;
+            ap.qout = &xatt;                   // wo's activation quantisation, off the critical path
+            enqueue_attention(f, l, ap, sb);
         }
         B200_CUDA_CHECK(cudaEventRecord(f->e_join, sb));
         if (!skip("up")) mmv(f, L.up, xm, f->up, f->FF, gelu, sa);                                               // :2389-2392
@@ -697,7 +695,7 @@ static void enqueue_eval_generic(b200_falcon * f, int N, int n_past, float theta
         launch_layernorm(f->inp, E, L.ln_mlp_g, L.ln_mlp_b, f->gen_nm, E, E, N, sa); f->launches++;                     // :2166-2185
         if (dual) { launch_layernorm(f->inp, E, L.ln_attn_g, L.ln_attn_b, f->gen_na, E, E, N, sa); f->launches++; }
         mm_any(f, L.wqkv, dual ? f->gen_na : f->gen_nm, N, f->qkv, f->QKV, false, sa);                                   // :2192
-        enqueue_attention(f, l, attn_params(f, l, N, n_past, graph_mode), theta_scale, sa);
+        enqueue_attention(f, l, attn_params(f, l, N, n_past, theta_scale, graph_mode), sa);
         mm_any(f, L.wo, f->att, N, f->ao, E, false, sa);                                                                 // :2370
         mm_any(f, L.up, f->gen_nm, N, f->up, FF, true, sa);                                                              // :2389-2392
         mm_any(f, L.down, f->up, N, f->dn, E, false, sa);                                                                // :2394
@@ -734,9 +732,9 @@ static void enqueue_eval(b200_falcon * f, int N, int n_past, float theta_scale, 
         B200_CUDA_CHECK(cudaEventRecord(f->e_join, sb));
         // attention branch on s_main
         mm(f, L.wqkv, dual ? xa : xm, N, f->qkv, f->QKV, EPI_NONE, f->xh_a, sa);                                   // :2192
-        AttnParams ap = attn_params(f, l, N, n_past, graph_mode);
-        if (N == 1) { ap.fuse_rope = 1; ap.rope_theta_scale = theta_scale; }                                    // decode: RoPE + KV append inside the attention launch
-        enqueue_attention(f, l, ap, theta_scale, sa);
+        AttnParams ap = attn_params(f, l, N, n_past, theta_scale, graph_mode);
+        ap.fuse_rope = N == 1;                                                                                   // decode: RoPE + KV append inside the attention kernels
+        enqueue_attention(f, l, ap, sa);
         launch_quantize_act(f->att, E, xatt, sa); f->launches++;
         mm(f, L.wo, xatt, N, f->ao, E, EPI_NONE, f->xh_a, sa);                                                  // :2370
         B200_CUDA_CHECK(cudaStreamWaitEvent(sa, f->e_join, 0));                                                  // join

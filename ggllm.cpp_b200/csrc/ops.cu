@@ -366,14 +366,12 @@ float rope_theta_scale_host(int head_dim, int n_ctx_rope, int dynamic_mode, floa
     } else if (ntk_alpha != 0.0f) alpha = powf(ntk_alpha, head_dim / (head_dim - 2.0));
     return powf(alpha * fb, -2.0f / head_dim);
 }
-// pair i of a head at position p: theta = p * theta_scale^i built by repeated fp32 multiplication, as the CPU loop does
+// pair i of a head at position p, in place
 __device__ __forceinline__ void rope_pair(float * v, int half, int i, int p, float theta_scale) {
-    float theta = (float) p;
-    for (int k = 0; k < i; k++) theta = __fmul_rn(theta, theta_scale);
+    const float theta = rope_theta(p, i, theta_scale);
     const float c = cosf(theta), s = sinf(theta);
-    const float x0 = v[i], x1 = v[i + half];
-    v[i] = __fsub_rn(__fmul_rn(x0, c), __fmul_rn(x1, s));
-    v[i + half] = __fadd_rn(__fmul_rn(x0, s), __fmul_rn(x1, c));
+    const float2 r = rope_rotate(v[i], v[i + half], c, s);
+    v[i] = r.x; v[i + half] = r.y;
 }
 __global__ void rope_neox_kernel(float * __restrict__ x, int n_head, int head_dim, int64_t tok_stride, int n_past, const int * __restrict__ n_past_dev, float theta_scale) {
     const int t = blockIdx.y, h = blockIdx.x, i = threadIdx.x;
@@ -421,8 +419,7 @@ __global__ void __launch_bounds__(256) rope_kv_append_batch_kernel(float * __res
         __shared__ float cs[64], sn[64];
         const int t = blockIdx.x, pos = n_past + t;
         if ((int) threadIdx.x < half) {
-            float theta = (float) pos;
-            for (int k = 0; k < (int) threadIdx.x; k++) theta = __fmul_rn(theta, theta_scale);
+            const float theta = rope_theta(pos, threadIdx.x, theta_scale);
             cs[threadIdx.x] = cosf(theta); sn[threadIdx.x] = sinf(theta);
         }
         __syncthreads();
@@ -430,8 +427,8 @@ __global__ void __launch_bounds__(256) rope_kv_append_batch_kernel(float * __res
         for (int idx = threadIdx.x; idx < (H + HKV) * half; idx += 256) {
             const int slot = idx / half, i = idx % half;
             float * v = row + (size_t) slot * D;
-            const float x0 = v[i], x1 = v[i + half], c = cs[i], s = sn[i];
-            const float r0 = __fsub_rn(__fmul_rn(x0, c), __fmul_rn(x1, s)), r1 = __fadd_rn(__fmul_rn(x0, s), __fmul_rn(x1, c));
+            const float2 r = rope_rotate(v[i], v[i + half], cs[i], sn[i]);
+            const float r0 = r.x, r1 = r.y;
             v[i] = r0; v[i + half] = r1;
             if (slot >= H) {
                 const size_t o = ((size_t) pos * HKV + (slot - H)) * D;
