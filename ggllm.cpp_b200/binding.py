@@ -24,7 +24,8 @@ PART_B = ["b200_falcon_create", "b200_falcon_set_tensor", "b200_falcon_set_tenso
           "b200_ggcc_read_hparams", "b200_falcon_free", "b200_falcon_weight_bytes", "b200_nccl_unique_id",
           "b200_falcon_init_pipeline", "b200_falcon_eval", "b200_falcon_decode_dev", "b200_falcon_logits_dev", "b200_falcon_generate_greedy",
           "b200_falcon_last_launches", "b200_attention_long_launches", "b200_falcon_last_ms", "b200_falcon_stream", "b200_falcon_profile_matvec",
-          "b200_falcon_kv_read", "b200_falcon_kv_write", "b200_falcon_kv_shadow_read", "b200_falcon_kv_fill_random", "b200_falcon_generate", "b200_falcon_generate_chain", "b200_falcon_load_seconds", "b200_falcon_save_kv", "b200_falcon_load_kv"]
+          "b200_falcon_kv_read", "b200_falcon_kv_write", "b200_falcon_kv_shadow_read", "b200_falcon_kv_fill_random", "b200_falcon_generate", "b200_falcon_generate_chain", "b200_falcon_load_seconds", "b200_falcon_save_kv", "b200_falcon_load_kv",
+          "b200_falcon_tap", "b200_falcon_tap_read"]
 
 
 def build(verbose=False):
@@ -79,6 +80,7 @@ def lib():
             "b200_falcon_eval": (i32, [vp, vp, i32, i32, i32, vp, i32]), "b200_falcon_decode_dev": (i32, [vp, vp, i32, i32]), "b200_falcon_generate_greedy": (i32, [vp, i32, i32, i32, i32, vp]),
             "b200_falcon_logits_dev": (vp, [vp]), "b200_falcon_last_launches": (i32, [vp]), "b200_falcon_last_ms": (f32, [vp]),
             "b200_falcon_stream": (vp, [vp]), "b200_falcon_profile_matvec": (f32, [vp, i32, vp, vp]),
+            "b200_falcon_tap": (i32, [vp, i32]), "b200_falcon_tap_read": (i32, [vp, i32, C.c_char_p, vp, sz]),
         }
         for name, (res, args) in sig.items():
             fn = getattr(L, name)
@@ -399,6 +401,18 @@ class Falcon:
         if self.L.b200_falcon_kv_shadow_read(self.h, layer, pos, n, _np_ptr(k), _np_ptr(vt)) != 0:
             raise RuntimeError("b200_falcon_kv_shadow_read: no fp16 copy, bad layer or range")
         return k, vt
+
+    def tap(self, on=True):
+        """switch the test tap on (copies of every layer's intermediates, b200_falcon_tap) or off"""
+        if self.L.b200_falcon_tap(self.h, int(bool(on))) != 0:
+            raise RuntimeError("b200_falcon_tap failed")
+
+    def tap_read(self, layer, node, dtype, shape):
+        """-> one tapped buffer of the most recent eval (layer -1: after the head) as an array of `dtype` and `shape`"""
+        out = np.empty(shape, dtype)
+        if self.L.b200_falcon_tap_read(self.h, layer, node.encode(), _np_ptr(out), out.nbytes) != 0:
+            raise KeyError("b200_falcon_tap_read: no node %r of layer %d with %d bytes" % (node, layer, out.nbytes))
+        return out
 
     def save_kv(self, path, n_tokens):
         if self.L.b200_falcon_save_kv(self.h, path.encode(), n_tokens) != 0:

@@ -318,11 +318,13 @@ size_t attention_scratch_bytes(const AttnParams & p) {
 }
 
 int launch_attention(float * qkv, float * k_cache, float * v_cache, float * out, int64_t out_stride, const AttnParams & p, float * scratch,
-                     cudaStream_t stream, bool * folded) {
+                     cudaStream_t stream, bool * folded, bool * rope_in_place) {
     if (folded) *folded = false;
+    if (rope_in_place) *rope_in_place = false;
     if (p.n_tok <= 0) return 0;
     const int tier = p.n_tok == 1 ? split_tier(p) : 0;
     int n = 0;
+    if (rope_in_place) *rope_in_place = !tier || !p.fuse_rope;
     if (!tier || !p.fuse_rope) { launch_rope_kv_append(qkv, k_cache, v_cache, p, p.rope_theta_scale, stream); n++; }       // in place
     bool fold = false;
     if (tier) {

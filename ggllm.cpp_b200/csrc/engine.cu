@@ -103,6 +103,11 @@ struct b200_falcon {
     double load_seconds = 0.0; size_t load_bytes = 0;   // b200_falcon_load_ggcc
     size_t pending_floats = 0;                  // logits of the eval in flight (falcon_eval_begin / finish)
     std::vector<const void *> borrowed;         // device planes adopted from another owner (ggml_cuda_transform_tensor): never freed here
+    // test tap (b200_falcon_tap): while mem is set, every eval copies its intermediates into mem -- one slice of layer_bytes per local
+    // layer at the end of that layer, then one slice after the head.  Node offsets are the same in every layer slice.
+    struct TapNode { std::string name; const void * src; size_t row_bytes, off; bool all_rows; };    // all_rows: N rows, else the head's rows
+    struct Tap { uint8_t * mem = nullptr; std::vector<TapNode> layer, head; size_t layer_bytes = 0; int rows = 0, head_rows = 0;
+                 std::vector<int> rotated; } tap;                // rotated[l]: RoPE ran in place on qkv (not inside the attention kernels)
 };
 
 // Local layer l's slice of the KV cache.  k / v: [n_ctx][n_head_kv][head_dim] f32, rows of kv_row() floats.  k16 / vt16: its fp16
@@ -497,7 +502,7 @@ void b200_falcon_free(b200_falcon * f) {
     cudaFree(f->lnf_g); cudaFree(f->lnf_b); cudaFree(f->k_cache); cudaFree(f->v_cache); cudaFree(f->k16); cudaFree(f->vt16);
     cudaFree(f->inp); cudaFree(f->qkv); cudaFree(f->att); cudaFree(f->ao); cudaFree(f->up); cudaFree(f->dn); cudaFree(f->logits);
     cudaFree(f->attn_scratch); cudaFree(f->actq_mem); cudaFree(f->gen_na); cudaFree(f->gen_nm); cudaFree(f->gen_actq); cudaFree(f->gen_xh); cudaFree(f->xh_a); cudaFree(f->xh_b); cudaFree(f->xh_m);
-    cudaFree(f->tokens_dev); cudaFree(f->n_past_dev); cudaFree(f->q_ctr); cudaFree(f->attn_dec_scratch);
+    cudaFree(f->tokens_dev); cudaFree(f->n_past_dev); cudaFree(f->q_ctr); cudaFree(f->attn_dec_scratch); cudaFree(f->tap.mem);
     cudaFreeHost(f->tokens_h); cudaFreeHost(f->n_past_h); cudaFreeHost(f->logits_h);
     for (auto & tier : f->graph) for (auto & g : tier) if (g.exec) cudaGraphExecDestroy(g.exec);
     cudaFree(f->tok_next); cudaFree(f->gen_hist); cudaFree(f->gen_step); cudaFree(f->sampler_work); sampler_state_free(f->sampler);
@@ -545,6 +550,23 @@ static void mm_any(b200_falcon * f, const WPlanes & W, const float * x, int N, f
     if (gelu) { B200_ASSERT(y_stride == W.M); launch_gelu(y, y, (int64_t) N * W.M, st); f->launches++; }                // ggml.c:10298-10337
 }
 
+// Test tap: D2D copies on s_main, after everything that writes the tapped buffers and before anything overwrites them.  Off (no mem):
+// nothing is enqueued.
+static void tap_copy(b200_falcon * f, const std::vector<b200_falcon::TapNode> & nodes, uint8_t * dst) {
+    for (const auto & n : nodes)
+        B200_CUDA_CHECK(cudaMemcpyAsync(dst + n.off, n.src, n.row_bytes * (n.all_rows ? f->tap.rows : f->tap.head_rows), cudaMemcpyDeviceToDevice, f->s_main));
+}
+static void tap_layer(b200_falcon * f, int l, int N) {
+    if (!f->tap.mem) return;
+    f->tap.rows = N;
+    tap_copy(f, f->tap.layer, f->tap.mem + (size_t) l * f->tap.layer_bytes);
+}
+static void tap_head(b200_falcon * f, int N, int nr) {
+    if (!f->tap.mem) return;
+    f->tap.rows = N; f->tap.head_rows = nr;
+    tap_copy(f, f->tap.head, f->tap.mem + (size_t) f->NL * f->tap.layer_bytes);
+}
+
 // final LayerNorm + lm_head over rows x[0 .. nr) of the residual stream: libfalcon.cpp:2422-2440.  ra / rb (optional, quantised head
 // only): the last layer's branch outputs, which the LayerNorm kernel adds to x first (x = (ra + rb) + x, written back)
 static void enqueue_head(b200_falcon * f, float * x, int nr, const float * ra, const float * rb, cudaStream_t sa) {
@@ -589,6 +611,7 @@ static void eval_output(b200_falcon * f, int N, int logits_rows_from, bool fold_
     if (f->NL > 0 && !fold) { launch_add3(f->dn, f->ao, f->inp, f->inp, (int64_t) N * f->E, f->s_main); f->launches++; }
     if (!f->last) { B200_NCCL_CHECK(nccl().Send(f->inp, (size_t) N * f->E, ncclFloat, f->hp.rank + 1, f->comm, f->s_main)); return; }
     enqueue_head(f, f->inp + (size_t) logits_rows_from * f->E, N - logits_rows_from, fold ? f->dn : nullptr, fold ? f->ao : nullptr, f->s_main);
+    tap_head(f, N, N - logits_rows_from);
     ring_token_out(f);
 }
 
@@ -615,7 +638,9 @@ static void enqueue_attention(b200_falcon * f, int l, const AttnParams & ap, cud
         }
         scratch = f->attn_scratch;
     }
-    f->launches += launch_attention(f->qkv, kv.k, kv.v, f->att, f->E, ap, scratch, st);
+    bool rotated = true;
+    f->launches += launch_attention(f->qkv, kv.k, kv.v, f->att, f->E, ap, scratch, st, nullptr, &rotated);
+    if (f->tap.mem) f->tap.rotated[l] = rotated;
 }
 
 static bool fused_decode_ok(const b200_falcon * f) {
@@ -678,6 +703,7 @@ static void enqueue_decode_fused(b200_falcon * f, int n_past, float theta_scale,
         B200_CUDA_CHECK(cudaStreamWaitEvent(sa, f->e_join, 0));
         if (!skip("wo")) mmv(f, L.wo, xatt, f->ao, E, wo_epi, sa);                                            // :2370
         if (wo_first && !skip("down")) mmv(f, L.down, xup, f->dn, E, none, sa);
+        tap_layer(f, l, 1);
     }
     eval_output(f, 1, 0, true);                                                      // :2399-2400, 2422-2440
 }
@@ -699,6 +725,7 @@ static void enqueue_eval_generic(b200_falcon * f, int N, int n_past, float theta
         mm_any(f, L.wo, f->att, N, f->ao, E, false, sa);                                                                 // :2370
         mm_any(f, L.up, f->gen_nm, N, f->up, FF, true, sa);                                                              // :2389-2392
         mm_any(f, L.down, f->up, N, f->dn, E, false, sa);                                                                // :2394
+        tap_layer(f, l, N);
     }
     eval_output(f, N, logits_rows_from, false);
 }
@@ -738,6 +765,7 @@ static void enqueue_eval(b200_falcon * f, int N, int n_past, float theta_scale, 
         launch_quantize_act(f->att, E, xatt, sa); f->launches++;
         mm(f, L.wo, xatt, N, f->ao, E, EPI_NONE, f->xh_a, sa);                                                  // :2370
         B200_CUDA_CHECK(cudaStreamWaitEvent(sa, f->e_join, 0));                                                  // join
+        tap_layer(f, l, N);
     }
     eval_output(f, N, logits_rows_from, false);
 }
@@ -1007,6 +1035,73 @@ int b200_falcon_load_kv(b200_falcon * f, const char * path) {
     fclose(fp);
     return n;
 }
+// Test tap: see include/ggml_b200.h.  The node list follows what ensure_actq allocated for this model (tensors must be set first).
+static void tap_add(std::vector<b200_falcon::TapNode> & v, size_t & total, const std::string & name, const void * src, size_t row_bytes,
+                    int NB, bool all_rows = true) {
+    if (!src) return;
+    v.push_back({ name, src, row_bytes, total, all_rows });
+    total += ((size_t) NB * row_bytes + 255) & ~(size_t) 255;
+}
+static void tap_add_actq(std::vector<b200_falcon::TapNode> & v, size_t & total, const std::string & name, const ActQ & A, int NB, bool all_rows = true) {
+    if (!A.q) return;
+    tap_add(v, total, name + ".q", A.q, (size_t) A.K, NB, all_rows);
+    tap_add(v, total, name + ".d", A.d, (size_t) (A.K / act_block(A.type)) * 4, NB, all_rows);
+    tap_add(v, total, name + ".s", A.s, (size_t) (A.K / 32) * 4, NB, all_rows);
+    tap_add(v, total, name + ".bs", A.bs, (size_t) (A.K / (A.type == T_Q8_K ? 16 : 32)) * 2, NB, all_rows);
+}
+int b200_falcon_tap(b200_falcon * f, int on) {
+    invalidate_graphs(f);                                 // the captured decode graphs hold the copies (or their absence)
+    B200_CUDA_CHECK(cudaDeviceSynchronize());
+    B200_CUDA_CHECK(cudaFree(f->tap.mem));
+    f->tap = b200_falcon::Tap{};
+    if (!on) return 0;
+    ensure_actq(f);
+    const int NB = f->hp.n_batch > 0 ? f->hp.n_batch : 1;
+    const size_t E4 = (size_t) f->E * 4;
+    auto & T = f->tap;
+    size_t lb = 0, hb = 0;
+    tap_add(T.layer, lb, "inp", f->inp, E4, NB); tap_add(T.layer, lb, "qkv", f->qkv, (size_t) f->QKV * 4, NB);
+    tap_add(T.layer, lb, "att", f->att, E4, NB); tap_add(T.layer, lb, "up", f->up, (size_t) f->FF * 4, NB);
+    tap_add(T.layer, lb, "dn", f->dn, E4, NB);   tap_add(T.layer, lb, "ao", f->ao, E4, NB);
+    if (f->act_type >= 0) {
+        tap_add_actq(T.layer, lb, "xa", f->xa, NB); tap_add_actq(T.layer, lb, "xm", f->xm, NB);
+        tap_add_actq(T.layer, lb, "xatt", f->xatt, NB); tap_add_actq(T.layer, lb, "xup", f->xup, NB);
+        tap_add(T.layer, lb, "xh_a", f->xh_a, (size_t) f->E * 2, NB); tap_add(T.layer, lb, "xh_b", f->xh_b, (size_t) f->FF * 2, NB);
+        tap_add(T.layer, lb, "xh_m", f->xh_m, (size_t) f->E * 2, NB);
+    }
+    if (f->generic_layers) { tap_add(T.layer, lb, "gen_na", f->gen_na, E4, NB); tap_add(T.layer, lb, "gen_nm", f->gen_nm, E4, NB); }
+    if (f->last) {
+        tap_add(T.head, hb, "inp", f->inp, E4, NB);
+        if (f->generic_head) tap_add(T.head, hb, "gen_na", f->gen_na, E4, NB, false);
+        else tap_add_actq(T.head, hb, "xf", f->xf, NB, false);
+        tap_add(T.head, hb, "logits", f->logits, (size_t) f->V * 4, NB, false);
+    }
+    T.layer_bytes = lb;
+    B200_CUDA_CHECK(cudaMalloc(&T.mem, lb * f->NL + hb + 256));
+    T.rotated.assign(f->NL, 0);
+    return 0;
+}
+int b200_falcon_tap_read(const b200_falcon * f, int layer, const char * node, void * host, size_t bytes) {
+    const auto & T = f->tap;
+    if (!T.mem || !node || !host) return 1;
+    const bool head = layer == -1;
+    const int l = layer - f->hp.layer_first;
+    if (head ? !f->last : (l < 0 || l >= f->NL)) return 1;
+    if (!head && !strcmp(node, "qkv_rotated")) {
+        if (bytes != sizeof(int)) return 1;
+        memcpy(host, &T.rotated[l], sizeof(int));
+        return 0;
+    }
+    for (const auto & n : head ? T.head : T.layer) {
+        if (n.name != node) continue;
+        if (bytes != n.row_bytes * (n.all_rows ? T.rows : T.head_rows)) return 1;
+        B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
+        B200_CUDA_CHECK(cudaMemcpy(host, T.mem + (head ? (size_t) f->NL * T.layer_bytes : (size_t) l * T.layer_bytes) + n.off, bytes, cudaMemcpyDeviceToHost));
+        return 0;
+    }
+    return 1;
+}
+
 int b200_falcon_last_launches(const b200_falcon * f) { return f->launches; }
 float b200_falcon_last_ms(const b200_falcon * f) { return f->last_ms; }
 void * b200_falcon_stream(b200_falcon * f) { return (void *) f->s_main; }

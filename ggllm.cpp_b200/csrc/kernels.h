@@ -87,9 +87,10 @@ int    attention_long_threshold();          // keys above which decode attention
 void   launch_rope_kv_append(float * qkv, float * k_cache, float * v_cache, const AttnParams & p, float theta_scale, cudaStream_t stream);
 // RoPE + KV append, then out[t][h*head_dim + i] = softmax(scale * Q K^T + causal mask) V   (libfalcon.cpp:2229-2366), and p.qout.
 // scratch: attention_scratch_bytes(p) bytes (null when that is 0).  Returns the number of kernels launched; folded (optional): whether
-// p.qout was written by the attention kernels themselves rather than by a quantize_act of its own.
+// p.qout was written by the attention kernels themselves rather than by a quantize_act of its own; rope_in_place (optional): whether
+// Q and K were rotated in qkv itself (false when the split-KV kernels did RoPE in registers, p.fuse_rope).
 int    launch_attention(float * qkv, float * k_cache, float * v_cache, float * out, int64_t out_stride, const AttnParams & p, float * scratch,
-                        cudaStream_t stream, bool * folded = nullptr);
+                        cudaStream_t stream, bool * folded = nullptr, bool * rope_in_place = nullptr);
 size_t attention_scratch_bytes(const AttnParams & p);                // one token: enough for either decode tier at any position
 int    attention_ctx_pad(int n_ctx);
 size_t attention_shadow_halves(int n_head_kv, int n_ctx);           // halves per layer, for k16 and for vt16 each

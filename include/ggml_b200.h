@@ -260,6 +260,25 @@ void *        b200_falcon_stream(b200_falcon * f);
  * `reps` passes, timed with CUDA events on the eval stream.  Returns total ms; fills the launch count and the
  * algorithmic weight bytes streamed in that region. */
 float         b200_falcon_profile_matvec(b200_falcon * f, int reps, int * n_launches, size_t * bytes);
+/* test hooks: the engine's intermediates.  b200_falcon_tap(f, 1) (after the tensors are set) allocates a tap arena with one slice per
+ * local layer, sized for n_batch tokens; while it is on, every eval (eager or captured decode graph) also enqueues device-to-device
+ * copies of its buffers into it on the eval stream: at the end of each layer, after both branches are complete and before the next
+ * layer's LayerNorm overwrites anything, and once after the head.  b200_falcon_tap(f, 0) frees it; with the tap off nothing is enqueued.
+ * Either call drops the captured decode graphs (they hold the copies).
+ * b200_falcon_tap_read copies one tapped buffer of the most recent eval to the host; `bytes` must be its exact size.
+ *   layer = a local (global index) layer, nodes at its end:
+ *     "inp" the layer's input residual [N][n_embd] f32; "qkv" [N][(n_head + 2 n_head_kv) head_dim] f32 (RoPE applied in place or not,
+ *     see "qkv_rotated"); "att", "ao", "dn" [N][n_embd] f32; "up" [N][4 n_embd] f32 (after GELU);
+ *     quantised activations "xa", "xm", "xatt", "xup" (fused paths) as "<name>.q" int8 codes [N][K], ".d" f32 scales [N][K/blk],
+ *     ".s" f32 Q8_1 sums [N][K/32], ".bs" int16 block sums (b200_actq_download's layout);
+ *     prompt GEMM path: fp16 operand planes "xh_m" (xm's), "xh_b" (xup's), "xh_a" (xatt's at that point) [N][K];
+ *     generic path: "gen_na", "gen_nm" the fp32 LayerNorm outputs [N][n_embd];
+ *     "qkv_rotated" one int: 1 if RoPE rotated Q and K inside qkv, 0 if the attention kernels rotated them in registers.
+ *   layer = -1 (last rank), after the head: "inp" the final residual [N][n_embd]; "xf.*" (quantised head) or "gen_na" (generic head) and
+ *     "logits", each over the head's rows (the last one, or all N with all_logits).
+ * Returns 0, or non-zero for a tap that is off, an unknown node, a layer that is not local or a wrong size. */
+int           b200_falcon_tap(b200_falcon * f, int on);
+int           b200_falcon_tap_read(const b200_falcon * f, int layer, const char * node, void * host, size_t bytes);
 /* number of kernel launches (graph nodes) issued by the most recent eval on this rank */
 int           b200_falcon_last_launches(const b200_falcon * f);
 int           b200_attention_long_launches(void);     /* diagnostics: launches (eager or captured) of the long-context decode attention kernels so far */

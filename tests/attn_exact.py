@@ -43,9 +43,11 @@ def _nearest_midpoint(x):
     return np.where(use_up, du, dd), np.where(use_up, up64, dn64)
 
 
-def reference(q, K, V, n_past, kind, vis_offset=0, drop_key=None, v_swap_key=None):
+def reference(q, K, V, n_past, kind, vis_offset=0, drop_key=None, v_swap_key=None, q_err=None):
     """q: [n_tok][n_head][64] rotated query rows (float32), K, V: [>= T][n_head_kv][64] cache rows with the new tokens' rows appended,
     T = n_past + n_tok; query token t sees keys [0, n_past + t + 1).  -> (out, bound), float64 [n_tok][n_head][64].
+    q_err: [n_tok][n_head][64] bound on |kernel's q - q| per element, for kernels that rotate Q themselves; it moves each score by at
+    most 0.125 sum_i q_err_i |k_i|, which joins the score error ds (and so the flip windows).
     Mutations that the sensitivity tests use to show the bound can fail: vis_offset widens every causal limit, drop_key hides one key
     from every row, v_swap_key takes that key's V row from the next KV head."""
     assert kind in KINDS
@@ -63,6 +65,7 @@ def reference(q, K, V, n_past, kind, vis_offset=0, drop_key=None, v_swap_key=Non
         if v_swap_key is not None:
             Vg[v_swap_key] = V[v_swap_key, (g + 1) % HKV]
         Qg = q[:, g * G:(g + 1) * G].reshape(n_tok * G, D).astype(np.float64)      # row = token * G + head in group
+        Eg = None if q_err is None else np.asarray(q_err, np.float64)[:, g * G:(g + 1) * G].reshape(n_tok * G, D)
         if kind == "ws":
             Qg, Kg, Vg = f16(Qg), f16(Kg), f16(Vg)
         absV = np.abs(Vg)
@@ -85,6 +88,8 @@ def reference(q, K, V, n_past, kind, vis_offset=0, drop_key=None, v_swap_key=Non
             else:   # hi x lo + lo x hi + hi x hi: the dropped lo x lo term and the split's own error 2^-22 |x| (or 2^-25 below 0.125)
                 ds = 0.125 * ((3 * 2.0 ** -22 + 16 * U23) * sabs
                               + 2.0 ** -25 * (np.abs(Qr).sum(1)[:, None] + np.abs(Kg).sum(1)[None, :]))
+            if Eg is not None:
+                ds = ds + 0.125 * (Eg[r0:r0 + 1024] @ np.abs(Kg).T)
             s = np.where(mask, s, -np.inf)
             m = s.max(1, keepdims=True)
             ds_m = np.take_along_axis(ds, s.argmax(1)[:, None], 1)
