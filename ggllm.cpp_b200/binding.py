@@ -19,7 +19,8 @@ PART_A = ["b200_event_create", "b200_event_destroy", "b200_event_record", "b200_
           "b200_weight_free", "b200_weight_device_bytes", "b200_dequantize_rows", "b200_actq_alloc", "b200_actq_free",
           "b200_quantize_act", "b200_actq_download", "b200_actq_alloc_f16", "b200_actq_download_f16", "b200_actq_to_f16", "b200_mul_mat", "b200_mul_mat_f16", "b200_mul_mat_vec_q", "b200_mul_mat_vec_q_chain", "b200_quantize_weights", "b200_mmv_max_n", "b200_mmv_launch_shape", "b200_layernorm",
           "b200_gelu", "b200_add", "b200_rope_neox", "b200_attention", "b200_layernorm_q", "b200_attention_decode",
-          "b200_sampler_create", "b200_sampler_create_chain", "b200_sampler_sample", "b200_sampler_mirostat_mu", "b200_sampler_free"]
+          "b200_sampler_create", "b200_sampler_create_chain", "b200_sampler_sample", "b200_sampler_mirostat_mu", "b200_sampler_free",
+          "b200_sampler_tap", "b200_sampler_tap_read"]
 PART_B = ["b200_falcon_create", "b200_falcon_set_tensor", "b200_falcon_set_tensor_random", "b200_falcon_load_ggcc",
           "b200_ggcc_read_hparams", "b200_falcon_free", "b200_falcon_weight_bytes", "b200_nccl_unique_id",
           "b200_falcon_init_pipeline", "b200_falcon_eval", "b200_falcon_decode_dev", "b200_falcon_logits_dev", "b200_falcon_generate_greedy",
@@ -68,6 +69,7 @@ def lib():
             "b200_falcon_kv_fill_random": (i32, [vp, i32, i32, C.c_uint64]),
             "b200_sampler_create": (vp, [vp, vp, i32]), "b200_sampler_sample": (i32, [vp, vp, i32]), "b200_sampler_free": (None, [vp]),
             "b200_sampler_create_chain": (vp, [vp, vp, i32]), "b200_sampler_mirostat_mu": (f32, [vp]),
+            "b200_sampler_tap": (i32, [vp, i32]), "b200_sampler_tap_read": (i32, [vp, C.c_char_p, C.c_char_p, vp, sz]),
             "b200_falcon_generate": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, vp]),
             "b200_falcon_generate_chain": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, vp]),
             "b200_falcon_load_seconds": (C.c_double, [vp, vp]),
@@ -276,6 +278,37 @@ class Sampler:
 
     def mirostat_mu(self):
         return float(self.L.b200_sampler_mirostat_mu(self.h))
+
+    def tap(self, on=True):
+        """switch the stage tap on (copies of the candidate list after every stage, b200_sampler_tap) or off"""
+        if self.L.b200_sampler_tap(self.h, int(bool(on))) != 0:
+            raise RuntimeError("b200_sampler_tap failed")
+
+    def _tap_field(self, stage, field, dtype, count):
+        out = np.empty(count, dtype)
+        if self.L.b200_sampler_tap_read(self.h, stage.encode(), field.encode(), _np_ptr(out), out.nbytes) != 0:
+            raise KeyError("b200_sampler_tap_read: no field %r of stage %r with %d bytes" % (field, stage, out.nbytes))
+        return out
+
+    def tap_stages(self, n_vocab):
+        """every stage of the most recent sample: {stage: {field: value}}; a stage that did not run has n = -1 only"""
+        st = {"row": {"n": n_vocab, "logits": self._tap_field("row", "logits", np.float32, n_vocab)}}
+        for stage in ("order", "tfs", "typical", "top_p", "temp", "final"):
+            n = int(self._tap_field(stage, "n", np.int32, 1)[0])
+            d = st[stage] = {"n": n}
+            if n < 0:
+                continue
+            d["ids"] = self._tap_field(stage, "ids", np.int32, n)
+            d["logits"] = self._tap_field(stage, "logits", np.float32, n)
+            if stage not in ("order", "temp"):
+                d["p"] = self._tap_field(stage, "p", np.float32, n)
+        st["typical"]["entropy"] = np.float32(self._tap_field("typical", "entropy", np.float32, 1)[0])
+        f = st["final"]
+        f["u"] = float(self._tap_field("final", "u", np.float64, 1)[0])
+        for k in ("pick", "id", "k"):
+            f[k] = int(self._tap_field("final", k, np.int32, 1)[0])
+        f["mu"] = np.float32(self._tap_field("final", "mu", np.float32, 1)[0])
+        return st
 
     def free(self):
         if self.h:

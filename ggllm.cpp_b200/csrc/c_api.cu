@@ -267,12 +267,15 @@ bool sampler_params_of(const b200_sampling_chain * c, int n_vocab, SamplerParams
     *out = p;
     return true;
 }
-struct b200_sampler { SamplerState * st; SamplerParams p; float * work; size_t work_floats; int32_t * out; };
+struct b200_sampler {
+    SamplerState * st; SamplerParams p; float * work; size_t work_floats; int32_t * out;
+    bool tap_on; float * tap; size_t tap_bytes; int tap_vocab;          // b200_sampler_tap: the arena, sized lazily like work
+};
 b200_sampler * b200_sampler_create_chain(const b200_sampling_chain * c, const int32_t * last_tokens, int n_last) {
     SamplerParams p;
     if (!sampler_params_of(c, -1, &p) || n_last < 0 || (n_last > 0 && !last_tokens)) return nullptr;
     b200_sampler * s = new b200_sampler();
-    s->st = sampler_state_alloc(); s->p = p; s->work = nullptr; s->work_floats = 0;
+    s->st = sampler_state_alloc(); s->p = p; s->work = nullptr; s->work_floats = 0; s->tap_on = false; s->tap = nullptr; s->tap_bytes = 0; s->tap_vocab = 0;
     B200_CUDA_CHECK(cudaMalloc(&s->out, 4));
     int32_t * w = nullptr;
     if (n_last > 0) { B200_CUDA_CHECK(cudaMalloc(&w, (size_t) n_last * 4)); B200_CUDA_CHECK(cudaMemcpyAsync(w, last_tokens, (size_t) n_last * 4, cudaMemcpyHostToDevice, g_stream)); }
@@ -293,16 +296,33 @@ int32_t b200_sampler_sample(b200_sampler * s, const float * logits_dev, int n_vo
         if (s->work) B200_CUDA_CHECK(cudaFree(s->work));
         s->work_floats = sampler_work_floats(n_vocab); B200_CUDA_CHECK(cudaMalloc(&s->work, s->work_floats * 4));
     }
+    if (s->tap_on && sampler_tap_bytes(n_vocab) > s->tap_bytes) {
+        if (s->tap) B200_CUDA_CHECK(cudaFree(s->tap));
+        s->tap_bytes = sampler_tap_bytes(n_vocab); B200_CUDA_CHECK(cudaMalloc(&s->tap, s->tap_bytes));
+    }
+    s->tap_vocab = n_vocab;
     SamplerParams p = s->p;
     if (p.top_k > n_vocab) p.top_k = n_vocab;
-    launch_sample(logits_dev, n_vocab, p, s->st, s->work, s->out, nullptr, nullptr, g_stream);
+    launch_sample(logits_dev, n_vocab, p, s->st, s->work, s->out, nullptr, nullptr, s->tap_on ? s->tap : nullptr, g_stream);
     int32_t id = -1;
     B200_CUDA_CHECK(cudaMemcpyAsync(&id, s->out, 4, cudaMemcpyDeviceToHost, g_stream));
     B200_CUDA_CHECK(cudaStreamSynchronize(g_stream));
     return id;
 }
 float b200_sampler_mirostat_mu(const b200_sampler * s) { B200_CUDA_CHECK(cudaStreamSynchronize(g_stream)); return sampler_mu(s->st); }
-void b200_sampler_free(b200_sampler * s) { if (!s) return; sampler_state_free(s->st); cudaFree(s->work); cudaFree(s->out); delete s; }
+void b200_sampler_free(b200_sampler * s) { if (!s) return; sampler_state_free(s->st); cudaFree(s->work); cudaFree(s->out); cudaFree(s->tap); delete s; }
+int b200_sampler_tap(b200_sampler * s, int on) {
+    if (!s) return 1;
+    B200_CUDA_CHECK(cudaStreamSynchronize(g_stream));
+    if (!on && s->tap) { B200_CUDA_CHECK(cudaFree(s->tap)); s->tap = nullptr; s->tap_bytes = 0; }
+    s->tap_on = on != 0; s->tap_vocab = 0;
+    return 0;
+}
+int b200_sampler_tap_read(const b200_sampler * s, const char * stage, const char * field, void * host, size_t bytes) {
+    if (!s || !s->tap || s->tap_vocab <= 0 || !stage || !field || !host) return 1;
+    B200_CUDA_CHECK(cudaStreamSynchronize(g_stream));
+    return sampler_tap_read(s->tap, s->tap_vocab, stage, field, host, bytes) ? 0 : 1;
+}
 
 // the decode step's LayerNorm node exactly as the engine launches it (cluster kernel for one row of <= 8192 values, register
 // kernel otherwise): [x = (ra + rb) + x] ; a1 = Q(norm(x) * g1 + b1) ; a2 = Q(norm(x) * g2 + b2) (a2 optional)

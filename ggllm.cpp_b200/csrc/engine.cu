@@ -589,7 +589,7 @@ static void enqueue_head(b200_falcon * f, float * x, int nr, const float * ra, c
 static void ring_token_out(b200_falcon * f) {
     if (!f->ring_mode) return;
     int32_t * dst = f->hp.world > 1 ? f->tok_next : f->tokens_dev;
-    if (f->use_sampler) launch_sample(f->logits, f->V, f->sampler_p, f->sampler, f->sampler_work, dst, f->gen_hist, f->gen_step, f->s_main);
+    if (f->use_sampler) launch_sample(f->logits, f->V, f->sampler_p, f->sampler, f->sampler_work, dst, f->gen_hist, f->gen_step, nullptr, f->s_main);
     else launch_argmax_hist(f->logits, f->V, dst, f->gen_hist, f->gen_step, f->s_main);
     f->launches++;
     if (f->hp.world > 1) B200_NCCL_CHECK(nccl().Send(f->tok_next, 1, ncclInt32, 0, f->comm, f->s_main));

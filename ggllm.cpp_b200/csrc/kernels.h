@@ -116,7 +116,11 @@ void   sampler_state_free(SamplerState * s);
 size_t sampler_work_floats(int n_vocab);                       // size of launch_sample's `work` scratch
 float  sampler_mu(const SamplerState * s);                     // synchronous read of the mirostat state
 void   launch_sampler_init(SamplerState * s, uint32_t seed, const int32_t * window_dev, int n, int cap, float mu, cudaStream_t stream);
-void   launch_sample(const float * logits, int n_vocab, const SamplerParams & p, SamplerState * st, float * work, int32_t * out, int32_t * hist, int * step, cudaStream_t stream);
+// tap: null, or sampler_tap_bytes(n_vocab) bytes that receive the candidate list after every stage (b200_sampler_tap)
+void   launch_sample(const float * logits, int n_vocab, const SamplerParams & p, SamplerState * st, float * work, int32_t * out, int32_t * hist, int * step,
+                     float * tap, cudaStream_t stream);
+size_t sampler_tap_bytes(int n_vocab);
+bool   sampler_tap_read(const float * tap, int n_vocab, const char * stage, const char * field, void * host, size_t bytes);
 
 // ---- engine.cu (internal, C++ linkage): adopt a matrix that is already resident in the planar layout (no copy, not freed by the engine)
 struct b200_falcon;

@@ -11,18 +11,25 @@
 //   otherwise   llama_sample_top_k (:3094-3118) -> tail_free (:3154-3203) -> typical (:3206-3267) -> top_p (:3121-3150, including its
 //               "last_idx = i" cut, which drops the candidate that crosses p) -> temperature (:3269-3279) -> llama_sample_token
 //               (:3449-3468): softmax in fp32, then std::discrete_distribution over the probabilities driven by the context's std::mt19937
-// is restated here bit for bit, INCLUDING the random draw: the kernel carries the MT19937 state (seeded like std::mt19937(seed)),
-// builds the double-precision cumulative table of libstdc++'s discrete_distribution (normalise by the double sum, partial sums, last
-// entry forced to 1.0), draws generate_canonical<double, 53> from two 32-bit outputs and takes the lower bound -- so a run with the
-// same seed samples the same ids as the reference, up to expf / logf / powf differing by an ulp between the device and glibc (a draw
-// or a cut within ~1e-7 of a boundary).
+// is restated here, INCLUDING the random draw: the kernel carries the MT19937 state (seeded like std::mt19937(seed)), builds the
+// double-precision cumulative table of libstdc++'s discrete_distribution (normalise by the double sum, partial sums, last entry
+// forced to 1.0), draws generate_canonical<double, 53> from two 32-bit outputs and takes the lower bound.
 //
 // Arithmetic: the reference is compiled with g++ -O3 -std=c++11 -march=x86-64-v3 (oracle/Makefile), where ISO mode turns fp
 // contraction off -- except that its objdump shows three fused multiply-adds, all in mirostat: sum_ti_bi and sum_ti_sq
 // (vfmadd231ss) and the mu update (vfnmadd213ss).  Those three use fmaf here; everything else is written with __f*_rn so that nvcc
 // cannot fuse it.  Every fp32 sum runs sequentially in the reference's order (softmax sums stop early once a term cannot change
-// the sum, see seq_sum_desc); logf / log2f / powf are evaluated in double and rounded once, which is what glibc's correctly-rounded-in-
-// practice float functions return.
+// the sum, see seq_sum_desc).
+//
+// Transcendentals: expf / logf / log2f / powf are evaluated in double and rounded once (ref_expf ...), i.e. correctly rounded
+// except within ~2^-29 relative of a float rounding boundary.  glibc's float functions are NOT correctly rounded: on an x86-64 host
+// with FMA (glibc 2.39) logf differs from the correctly rounded value on 0.73 % of probabilities in (0, 1), log2f on 0.56 %, expf
+// on 0.06 % of arguments in (-40, 0], powf on 0.06 % of pairs.  So the device is bit for bit with an exact restatement of the
+// chain over correctly rounded functions (tests/sampler_twin.py, checked stage by stage through the tap below), and the reference
+// differs from that restatement in the last bit of a probability, typical's entropy and scores, or mirostat's s_hat and mu
+// wherever glibc rounds differently.  An id changes only when such an ulp moves a value across a boundary (a draw, a cut or
+// mirostat 1's int(k)); over the 1,558 fixed-seed steps of tests/test_sampler_stages_gpu.py that count is zero.
+// Matching glibc bit for bit would mean carrying its float functions' tables onto the device, which this file does not do.
 //
 // Ordering: top-k with 1 <= k <= 1024 (the default chain) takes k rounds of block arg-max as before; mirostat, top_k <= 0 and
 // top_k > 1024 sort the whole row with a stable LSD radix sort (4 passes of 8 bits over an L2-resident scratch), descending logits
@@ -31,6 +38,7 @@
 // One CTA of 1024 threads; every sequential part runs on thread 0.
 #include "kernels.h"
 #include <climits>
+#include <cstring>
 
 struct SamplerState {                   // device resident
     uint32_t mt[624]; int mti;
@@ -66,7 +74,8 @@ __global__ void sampler_init_kernel(SamplerState * s, uint32_t seed, const int32
     s->mu = mu;
 }
 
-// glibc's logf / log2f / powf are correctly rounded in practice; double evaluation rounded once gives the same float
+// correctly rounded float transcendentals (double evaluation, rounded once); glibc's float functions differ in the last bit at times
+__device__ __forceinline__ float ref_expf(float x) { return (float) exp((double) x); }
 __device__ __forceinline__ float ref_logf(float x) { return (float) log((double) x); }
 __device__ __forceinline__ float ref_log2f(float x) { return (float) log2((double) x); }
 __device__ __forceinline__ float ref_powf(float x, float y) { return (float) pow((double) x, (double) y); }
@@ -95,7 +104,7 @@ __device__ float seq_sum_desc(const float * x, int n) {
 // desc: cl is in descending order, so the sum may stop early; after typical's reordering it may not.
 __device__ void block_softmax(const float * cl, float * cp, int n, float * s_f, bool desc = true) {
     const float mx = cl[0];
-    for (int i = threadIdx.x; i < n; i += NT) cp[i] = expf(__fsub_rn(cl[i], mx));
+    for (int i = threadIdx.x; i < n; i += NT) cp[i] = ref_expf(__fsub_rn(cl[i], mx));
     __syncthreads();
     if (threadIdx.x == 0) {
         if (desc) s_f[0] = seq_sum_desc(cp, n);
@@ -207,6 +216,11 @@ __device__ void block_radix_sort(uint32_t * k0, int32_t * v0, uint32_t * ka, int
     }
 }
 
+enum { TAP_ORDER, TAP_TFS, TAP_TYPICAL, TAP_TOP_P, TAP_TEMP, TAP_FINAL, TAP_STAGES };
+struct TapHead { int n[TAP_STAGES]; int pick, id, k; float entropy, mu; double u; };      // n = -1: the stage did not run
+constexpr int TAP_HEAD_FLOATS = 64;
+static_assert(sizeof(TapHead) <= TAP_HEAD_FLOATS * 4, "tap head");
+
 struct Scratch {                        // sampler_work_floats(n) floats, carved into n-entry arrays
     float * work; uint32_t * k0; uint32_t * ka; int32_t * v0; int32_t * va; int32_t * cid; float * cl; float * cp; float * tmp;
 };
@@ -217,8 +231,24 @@ __device__ __forceinline__ Scratch carve(float * w, int n) {
     return s;
 }
 
+// test tap (b200_sampler_tap): a copy of the candidate list after every stage, in the order the reference holds it.  Layout
+// (sampler_tap_bytes): the TapHead, then the row after bias and penalties [n_vocab], then per stage ids, logits, p [n_vocab] each.
+__device__ __forceinline__ int32_t * tap_ids(float * tap, int V, int stage) { return (int32_t *) (tap + TAP_HEAD_FLOATS + V + (size_t) (3 * stage) * V); }
+__device__ __forceinline__ float * tap_logits(float * tap, int V, int stage) { return tap + TAP_HEAD_FLOATS + V + (size_t) (3 * stage + 1) * V; }
+__device__ __forceinline__ float * tap_p(float * tap, int V, int stage) { return tap + TAP_HEAD_FLOATS + V + (size_t) (3 * stage + 2) * V; }
+// entry i is candidate perm[i] (perm null: i) of ids / l / p (p null: not written).  Called by every thread, in uniform control flow.
+__device__ void tap_list(float * tap, int V, int stage, int n, const int32_t * ids, const float * l, const float * p, const int32_t * perm) {
+    for (int i = threadIdx.x; i < n; i += NT) {
+        const int j = perm ? perm[i] : i;
+        tap_ids(tap, V, stage)[i] = ids[j]; tap_logits(tap, V, stage)[i] = l[j];
+        if (p) tap_p(tap, V, stage)[i] = p[j];
+    }
+    if (threadIdx.x == 0) ((TapHead *) tap)->n[stage] = n;
+    __syncthreads();
+}
+
 __global__ void __launch_bounds__(NT) sample_kernel(const float * __restrict__ logits, int n_vocab, SamplerParams p, SamplerState * st,
-                                                    float * __restrict__ work, int32_t * out, int32_t * hist, int * step) {
+                                                    float * __restrict__ work, int32_t * out, int32_t * hist, int * step, float * tap) {
     __shared__ float sv[32]; __shared__ int si[32];
     __shared__ int32_t win[B200_SAMPLER_MAX_WINDOW]; __shared__ int s_wlen;
     __shared__ int s_cnt[32][256]; __shared__ int s_base[256];
@@ -231,6 +261,11 @@ __global__ void __launch_bounds__(NT) sample_kernel(const float * __restrict__ l
     const int wlen = s_wlen;
     for (int i = tid; i < wlen; i += NT) win[i] = st->window[i];
     for (int i = tid; i < n_vocab; i += NT) S.work[i] = logits[i];
+    if (tap && tid == 0) {
+        TapHead * h = (TapHead *) tap;
+        for (int s = 0; s < TAP_STAGES; s++) h->n[s] = -1;
+        h->pick = -1; h->id = -1; h->k = -1; h->entropy = NAN; h->mu = st->mu; h->u = -1.0;
+    }
     __syncthreads();
     // ---- logit bias (ids unique, validated on the host), then the penalties on each distinct id of the window
     if (tid < p.n_bias) S.work[p.bias_id[tid]] = __fadd_rn(S.work[p.bias_id[tid]], p.bias_value[tid]);
@@ -247,11 +282,16 @@ __global__ void __launch_bounds__(NT) sample_kernel(const float * __restrict__ l
         }
     }
     __syncthreads();
+    if (tap) {
+        for (int i = tid; i < n_vocab; i += NT) tap[TAP_HEAD_FLOATS + i] = S.work[i];
+        __syncthreads();
+    }
     int n, pick = 0;
     bool reordered = false;                                            // typical left the candidates out of descending order
     const bool greedy = p.temp <= 0.f;
     if (greedy || (p.mirostat == 0 && p.top_k >= 1 && p.top_k <= NT)) {
-        // ---- the k largest logits, descending (equal values: lowest id first), by k rounds of block arg-max
+        // ---- the k largest logits, descending (equal values: lowest id first), by k rounds of block arg-max; a taken entry becomes
+        // NaN, so it cannot win again even when every entry left is -inf
         n = greedy ? 1 : min(p.top_k, n_vocab);
         for (int r = 0; r < n; r++) {
             float best = -INFINITY; int bi = 0x7fffffff;
@@ -270,7 +310,7 @@ __global__ void __launch_bounds__(NT) sample_kernel(const float * __restrict__ l
                     const float ov = __shfl_xor_sync(0xffffffffu, best, o); const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
                     if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
                 }
-                if (lane == 0) { S.cl[r] = best; S.cid[r] = bi; if (bi < n_vocab) S.work[bi] = -INFINITY; }
+                if (lane == 0) { S.cl[r] = best; S.cid[r] = bi; if (bi < n_vocab) S.work[bi] = NAN; }   // NaN loses every comparison
             }
             __syncthreads();
         }
@@ -287,6 +327,7 @@ __global__ void __launch_bounds__(NT) sample_kernel(const float * __restrict__ l
         __syncthreads();
         n = (p.mirostat != 0 || p.top_k <= 0 || p.top_k > n_vocab) ? n_vocab : p.top_k;
     }
+    if (tap) tap_list(tap, n_vocab, TAP_ORDER, n, S.cid, S.cl, nullptr, nullptr);
 
     if (!greedy && p.mirostat == 1) {
         block_softmax(S.cl, S.cp, n, s_f);
@@ -305,6 +346,7 @@ __global__ void __launch_bounds__(NT) sample_kernel(const float * __restrict__ l
             int ki = x86_float_to_int(k);
             ki = max(ki, 1); ki = min(ki, n);
             s_i[1] = ki;
+            if (tap) ((TapHead *) tap)->k = ki;
         }
         __syncthreads();
         n = s_i[1];
@@ -339,6 +381,7 @@ __global__ void __launch_bounds__(NT) sample_kernel(const float * __restrict__ l
             __syncthreads();
             n = s_i[1];
             __syncthreads();
+            if (tap) tap_list(tap, n_vocab, TAP_TFS, n, S.cid, S.cl, S.cp, nullptr);
         }
         // ---- typical: candidates reordered by |-log p - entropy| (ascending), cut where their probabilities pass typical_p
         if (p.typical_p < 1.0f) {
@@ -363,6 +406,10 @@ __global__ void __launch_bounds__(NT) sample_kernel(const float * __restrict__ l
             }
             __syncthreads();
             const int last = s_i[1];
+            if (tap) {
+                if (tid == 0) ((TapHead *) tap)->entropy = ent;
+                tap_list(tap, n_vocab, TAP_TYPICAL, last, S.cid, S.cl, S.cp, S.v0);
+            }
             for (int i = tid; i < last; i += NT) { const int j = S.v0[i]; S.va[i] = S.cid[j]; S.tmp[i] = S.cl[j]; }
             __syncthreads();
             for (int i = tid; i < last; i += NT) { S.cid[i] = S.va[i]; S.cl[i] = S.tmp[i]; }
@@ -383,9 +430,11 @@ __global__ void __launch_bounds__(NT) sample_kernel(const float * __restrict__ l
             __syncthreads();
             n = s_i[1];
             __syncthreads();
+            if (tap) tap_list(tap, n_vocab, TAP_TOP_P, n, S.cid, S.cl, S.cp, nullptr);
         }
         for (int i = tid; i < n; i += NT) S.cl[i] = __fdiv_rn(S.cl[i], p.temp);       // llama_sample_temperature
         __syncthreads();
+        if (tap) tap_list(tap, n_vocab, TAP_TEMP, n, S.cid, S.cl, nullptr, nullptr);
     }
     if (!greedy) {
         // ---- llama_sample_token: softmax, discrete_distribution(probs)(rng); mirostat then updates mu from the drawn p
@@ -397,6 +446,12 @@ __global__ void __launch_bounds__(NT) sample_kernel(const float * __restrict__ l
             const float e = __fsub_rn(-ref_log2f(S.cp[pick]), p.mirostat_tau);
             st->mu = fmaf(-p.mirostat_eta, e, st->mu);
         }
+        if (tap && tid == 0 && n >= 2) ((TapHead *) tap)->u = s_d[NT];
+    } else if (tid == 0) S.cp[0] = 1.0f;
+    if (tap) {
+        __syncthreads();
+        tap_list(tap, n_vocab, TAP_FINAL, n, S.cid, S.cl, S.cp, nullptr);
+        if (tid == 0) { TapHead * h = (TapHead *) tap; h->pick = pick; h->id = S.cid[pick]; h->mu = st->mu; }
     }
     if (tid != 0) return;
     const int id = S.cid[pick];
@@ -413,6 +468,35 @@ __global__ void __launch_bounds__(NT) sample_kernel(const float * __restrict__ l
 SamplerState * sampler_state_alloc() { SamplerState * s = nullptr; B200_CUDA_CHECK(cudaMalloc(&s, sizeof(SamplerState))); return s; }
 void sampler_state_free(SamplerState * s) { if (s) B200_CUDA_CHECK(cudaFree(s)); }
 size_t sampler_work_floats(int n_vocab) { return 9 * (size_t) n_vocab; }
+size_t sampler_tap_bytes(int n_vocab) { return 4 * (TAP_HEAD_FLOATS + (1 + 3 * (size_t) TAP_STAGES) * n_vocab); }
+// one stage of the tap (see tap_list) copied to the host; returns false for an unknown stage / field or a wrong size
+bool sampler_tap_read(const float * tap, int n_vocab, const char * stage, const char * field, void * host, size_t bytes) {
+    static const char * names[TAP_STAGES] = { "order", "tfs", "typical", "top_p", "temp", "final" };
+    TapHead h;
+    B200_CUDA_CHECK(cudaMemcpy(&h, tap, sizeof(h), cudaMemcpyDeviceToHost));
+    auto scalar = [&](const void * v, size_t sz) { if (bytes != sz) return false; memcpy(host, v, sz); return true; };
+    if (!strcmp(stage, "row")) {
+        if (strcmp(field, "logits") || bytes != (size_t) n_vocab * 4) return false;
+        B200_CUDA_CHECK(cudaMemcpy(host, tap + TAP_HEAD_FLOATS, bytes, cudaMemcpyDeviceToHost));
+        return true;
+    }
+    int s = 0;
+    while (s < TAP_STAGES && strcmp(stage, names[s])) s++;
+    if (s == TAP_STAGES) return false;
+    if (!strcmp(field, "n")) return scalar(&h.n[s], 4);
+    if (s == TAP_TYPICAL && !strcmp(field, "entropy")) return scalar(&h.entropy, 4);
+    if (s == TAP_FINAL) {
+        if (!strcmp(field, "u")) return scalar(&h.u, 8);
+        if (!strcmp(field, "pick")) return scalar(&h.pick, 4);
+        if (!strcmp(field, "id")) return scalar(&h.id, 4);
+        if (!strcmp(field, "mu")) return scalar(&h.mu, 4);
+        if (!strcmp(field, "k")) return scalar(&h.k, 4);
+    }
+    const int arr = !strcmp(field, "ids") ? 0 : !strcmp(field, "logits") ? 1 : !strcmp(field, "p") ? 2 : -1;
+    if (arr < 0 || (arr == 2 && (s == TAP_ORDER || s == TAP_TEMP)) || h.n[s] < 0 || bytes != (size_t) h.n[s] * 4) return false;
+    B200_CUDA_CHECK(cudaMemcpy(host, tap + TAP_HEAD_FLOATS + n_vocab + (size_t) (3 * s + arr) * n_vocab, bytes, cudaMemcpyDeviceToHost));
+    return true;
+}
 float sampler_mu(const SamplerState * s) {
     float mu = 0.f;
     B200_CUDA_CHECK(cudaMemcpy(&mu, &s->mu, 4, cudaMemcpyDeviceToHost));
@@ -424,8 +508,9 @@ void launch_sampler_init(SamplerState * s, uint32_t seed, const int32_t * window
     sampler_init_kernel<<<1, 1, 0, stream>>>(s, seed, window_dev, n, cap, mu);
     B200_CUDA_CHECK(cudaGetLastError());
 }
-void launch_sample(const float * logits, int n_vocab, const SamplerParams & p, SamplerState * st, float * work, int32_t * out, int32_t * hist, int * step, cudaStream_t stream) {
+void launch_sample(const float * logits, int n_vocab, const SamplerParams & p, SamplerState * st, float * work, int32_t * out, int32_t * hist, int * step,
+                   float * tap, cudaStream_t stream) {
     B200_ASSERT(p.mirostat >= 0 && p.mirostat <= 2 && p.n_bias >= 0 && p.n_bias <= B200_SAMPLER_MAX_BIAS);
-    sample_kernel<<<1, NT, 0, stream>>>(logits, n_vocab, p, st, work, out, hist, step);
+    sample_kernel<<<1, NT, 0, stream>>>(logits, n_vocab, p, st, work, out, hist, step, tap);
     B200_CUDA_CHECK(cudaGetLastError());
 }

@@ -153,7 +153,8 @@ int    b200_attention_decode(float * qkv_dev, float * k_cache_dev, float * v_cac
  * off, 0 the frequency / presence penalties.  Bad input is refused (NULL / 1): mirostat not 0..2, repeat_last_n outside 0..256,
  * n_logit_bias outside 0..B200_SAMPLER_MAX_BIAS, a bias id outside [0, n_vocab) or repeated, a NaN parameter.  Bias ids are
  * checked against n_vocab at every b200_sampler_sample (returns -1) and at b200_falcon_generate_chain.
- * The draw reproduces std::discrete_distribution over std::mt19937(seed), so the same seed samples the same ids as the reference. */
+ * The draw reproduces std::discrete_distribution over std::mt19937(seed), so the same seed samples the same ids as the reference,
+ * except where glibc's float functions, which are not correctly rounded, move a value across a boundary (sampling.cu). */
 typedef struct { int32_t top_k; float top_p; float temp; float repeat_penalty; int32_t repeat_last_n; uint32_t seed; } b200_sampling_params;
 #define B200_SAMPLER_MAX_BIAS 64
 typedef struct {
@@ -174,6 +175,22 @@ b200_sampler * b200_sampler_create_chain(const b200_sampling_chain * p, const in
 int32_t        b200_sampler_sample(b200_sampler * s, const float * logits_dev, int n_vocab);   /* samples, appends the id to the window, returns it */
 float          b200_sampler_mirostat_mu(const b200_sampler * s);                                /* mirostat's current mu */
 void           b200_sampler_free(b200_sampler * s);
+/* test hooks: the candidate list after every stage of the chain, in the order the reference's llama_sample_* functions leave it.
+ * b200_sampler_tap(s, 1) makes every later b200_sampler_sample also copy its stages into a tap arena on the device (allocated at the
+ * first sample, about 76 bytes per vocabulary entry); b200_sampler_tap(s, 0) frees it, and with the tap off nothing is copied.
+ * b200_sampler_tap_read copies one field of the most recent sample to the host; `bytes` must be its exact size.  Stages and fields:
+ *   "row"     logits [n_vocab] f32: after the logit bias and the penalties, in id order
+ *   "order"   n, ids, logits: after top-k's rounds or the whole-row sort (mirostat: after the division by temp)
+ *   "tfs"     n, ids, logits, p: after tail-free's cut; p is the softmax it cut on
+ *   "typical" n, ids, logits, p: after typical's reordering and cut; p as above; entropy (f32)
+ *   "top_p"   n, ids, logits, p: after top-p's cut
+ *   "temp"    n, ids, logits: after the division by temp (default chain)
+ *   "final"   n, ids, logits, p: the candidates of the draw and their probabilities; u (f64, the uniform variate; -1 when fewer
+ *             than two candidates draw nothing), pick (position drawn), id, mu (after mirostat's update), k (mirostat 1's cut, else -1)
+ * n, pick, id, k are int32 and the arrays hold n entries (ids int32, logits / p f32).  A stage that did not run has n = -1 and no
+ * arrays.  Both return 0 on success, 1 otherwise. */
+int            b200_sampler_tap(b200_sampler * s, int on);
+int            b200_sampler_tap_read(const b200_sampler * s, const char * stage, const char * field, void * host, size_t bytes);
 
 /* ========================================= part B: Falcon eval path ====================================== */
 

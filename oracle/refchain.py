@@ -12,6 +12,11 @@ def have_chain():
     return os.path.exists(LIB)
 
 
+def have_stages():
+    """the library exports refh_sample_chain_stages (a library built from an older ref_sample_chain.cpp does not)"""
+    return have_chain() and hasattr(C.CDLL(LIB), "refh_sample_chain_stages")
+
+
 def _p(a):
     return a.ctypes.data_as(C.c_void_p)
 
@@ -57,6 +62,32 @@ class RefChain:
                                        frequency_penalty, presence_penalty, mirostat, mirostat_tau, mirostat_eta, C.byref(m),
                                        ids.size, _p(ids), _p(vals))
         return int(tok), float(m.value)
+
+    STAGES = ("row", "order", "tfs", "typical", "top_p", "temp", "final")
+
+    def sample_chain_stages(self, logits, last_tokens, mu, top_k=40, top_p=0.95, tfs_z=1.0, typical_p=1.0, temp=0.8, repeat_penalty=1.1,
+                            frequency_penalty=0.0, presence_penalty=0.0, mirostat=0, mirostat_tau=5.0, mirostat_eta=0.1, logit_bias=None):
+        """-> (id, mu after the step, {stage: {"n", "ids", "logits", "p"}}): the candidates array after each llama_sample_* call of
+        refh_sample_chain (ref_sample_chain.cpp); a stage no call reached is absent"""
+        lg = np.ascontiguousarray(logits, np.float32)
+        lt = np.ascontiguousarray(last_tokens, np.int32)
+        ids = np.array(list((logit_bias or {}).keys()), np.int32)
+        vals = np.array(list((logit_bias or {}).values()), np.float32)
+        V = lg.size
+        sizes = np.empty(7, np.int32)
+        o_ids, o_l, o_p = np.empty(7 * V, np.int32), np.empty(7 * V, np.float32), np.empty(7 * V, np.float32)
+        f = self.L.refh_sample_chain_stages
+        f.restype, f.argtypes = C.c_int, self.L.refh_sample_chain.argtypes + [C.c_void_p] * 4
+        m = C.c_float(mu)
+        tok = f(self.h, _p(lg), V, _p(lt), lt.size, top_k, top_p, tfs_z, typical_p, temp, repeat_penalty,
+                                              frequency_penalty, presence_penalty, mirostat, mirostat_tau, mirostat_eta, C.byref(m),
+                                              ids.size, _p(ids), _p(vals), _p(sizes), _p(o_ids), _p(o_l), _p(o_p))
+        st = {}
+        for s, name in enumerate(self.STAGES):
+            n = int(sizes[s])
+            if n >= 0:
+                st[name] = dict(n=n, ids=o_ids[s * V:s * V + n].copy(), logits=o_l[s * V:s * V + n].copy(), p=o_p[s * V:s * V + n].copy())
+        return int(tok), float(m.value), st
 
     def close(self):
         if self.h:

@@ -12,9 +12,12 @@ CXXFLAGS_R= -O3 -std=c++11 -fPIC $(ARCH) -pthread $(REFDEFS) -I$(REF) -I$(REF)/e
 
 all: _ref/libfalcon_chain.so
 
-_ref/ref_sample_chain.o: ref_sample_chain.cpp
+# The harness and the library are remade on every build (one small file and a link): a prebuilt oracle/_ref copied into a checkout
+# is newer than the checked-out sources, so a timestamp rule would keep a library built from an older ref_sample_chain.cpp.
+_ref/ref_sample_chain.o: ref_sample_chain.cpp FORCE
 	$(CXX) $(CXXFLAGS_R) -c $< -o $@
-_ref/libfalcon_chain.so: _ref/ggml.o _ref/k_quants.o _ref/libfalcon.o _ref/cmpnct_unicode.o _ref/ref_harness.o _ref/ref_sample_chain.o
-	$(CXX) -shared -o $@ $^ -lm -pthread
+_ref/libfalcon_chain.so: _ref/ggml.o _ref/k_quants.o _ref/libfalcon.o _ref/cmpnct_unicode.o _ref/ref_harness.o _ref/ref_sample_chain.o FORCE
+	$(CXX) -shared -o $@ $(filter %.o,$^) -lm -pthread
 
-.PHONY: all
+FORCE:
+.PHONY: all FORCE
