@@ -18,10 +18,10 @@ PART_A = ["b200_event_create", "b200_event_destroy", "b200_event_record", "b200_
           "b200_memcpy_d2h", "b200_memset", "b200_host_malloc", "b200_host_free", "b200_weight_upload", "b200_weight_random",
           "b200_weight_free", "b200_weight_device_bytes", "b200_dequantize_rows", "b200_actq_alloc", "b200_actq_free",
           "b200_quantize_act", "b200_actq_download", "b200_actq_alloc_f16", "b200_actq_download_f16", "b200_actq_to_f16", "b200_mul_mat", "b200_mul_mat_f16", "b200_mul_mat_vec_q", "b200_mul_mat_vec_q_chain", "b200_quantize_weights", "b200_mmv_max_n", "b200_mmv_launch_shape", "b200_layernorm",
-          "b200_gelu", "b200_add", "b200_rope_neox", "b200_attention", "b200_layernorm_q", "b200_attention_decode",
+          "b200_gelu", "b200_add", "b200_rope_neox", "b200_attention", "b200_layernorm_q", "b200_attention_decode", "b200_attention_kv16", "b200_attention_decode_kv16",
           "b200_sampler_create", "b200_sampler_create_chain", "b200_sampler_sample", "b200_sampler_mirostat_mu", "b200_sampler_free",
           "b200_sampler_tap", "b200_sampler_tap_read"]
-PART_B = ["b200_falcon_create", "b200_falcon_set_tensor", "b200_falcon_set_tensor_random", "b200_falcon_load_ggcc",
+PART_B = ["b200_falcon_create", "b200_falcon_create_kv", "b200_falcon_kv_type", "b200_falcon_kv_device_bytes", "b200_falcon_set_tensor", "b200_falcon_set_tensor_random", "b200_falcon_load_ggcc",
           "b200_ggcc_read_hparams", "b200_falcon_free", "b200_falcon_weight_bytes", "b200_nccl_unique_id",
           "b200_falcon_init_pipeline", "b200_falcon_eval", "b200_falcon_decode_dev", "b200_falcon_logits_dev", "b200_falcon_generate_greedy",
           "b200_falcon_last_launches", "b200_attention_long_launches", "b200_falcon_last_ms", "b200_falcon_stream", "b200_falcon_profile_matvec",
@@ -64,6 +64,8 @@ def lib():
             "b200_attention": (None, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32]),
             "b200_layernorm_q": (None, [vp, i64, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32]),
             "b200_attention_decode": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]),
+            "b200_attention_kv16": (None, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32]),
+            "b200_attention_decode_kv16": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]),
             "b200_falcon_kv_read": (i32, [vp, i32, i32, i32, vp, vp]), "b200_falcon_kv_write": (i32, [vp, i32, i32, i32, vp, vp]),
             "b200_falcon_kv_shadow_read": (i32, [vp, i32, i32, i32, vp, vp]),
             "b200_falcon_kv_fill_random": (i32, [vp, i32, i32, C.c_uint64]),
@@ -74,7 +76,8 @@ def lib():
             "b200_falcon_generate_chain": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, vp]),
             "b200_falcon_load_seconds": (C.c_double, [vp, vp]),
             "b200_falcon_save_kv": (i32, [vp, C.c_char_p, i32]), "b200_falcon_load_kv": (i32, [vp, C.c_char_p]),
-            "b200_falcon_create": (vp, [vp]), "b200_falcon_set_tensor": (None, [vp, C.c_char_p, i32, i32, vp, vp]),
+            "b200_falcon_create": (vp, [vp]), "b200_falcon_create_kv": (vp, [vp, i32]), "b200_falcon_kv_type": (i32, [vp]),
+            "b200_falcon_kv_device_bytes": (sz, [vp]), "b200_falcon_set_tensor": (None, [vp, C.c_char_p, i32, i32, vp, vp]),
             "b200_falcon_set_tensor_random": (None, [vp, C.c_char_p, i32, C.c_uint64]),
             "b200_falcon_load_ggcc": (i32, [vp, C.c_char_p]), "b200_ggcc_read_hparams": (i32, [C.c_char_p, vp]),
             "b200_falcon_free": (None, [vp]), "b200_falcon_weight_bytes": (sz, [vp]),
@@ -337,14 +340,16 @@ def layer_range(n_layer, rank, world):
 class Falcon:
     """The Falcon eval path (include/ggml_b200.h part B)."""
 
-    def __init__(self, hp, n_ctx, n_batch=1, rank=0, world=1, layers=None):
+    def __init__(self, hp, n_ctx, n_batch=1, rank=0, world=1, layers=None, kv_f16=False):
+        """kv_f16: keep the KV cache in fp16 (b200_falcon_create_kv with GGML_TYPE_F16, the reference's f16_kv): half the cache bytes,
+        K / V rounded to fp16 as they are stored"""
         self.L = lib()
         self.hp = dict(hp)
         lf, ll = layers if layers is not None else layer_range(hp["n_layer"], rank, world)      # layers: an explicit (first, last) range, e.g. balanced by bytes
         self.params = FalconParams(hp["n_vocab"], hp["n_embd"], hp["n_head"], hp["n_head_kv"], hp["n_layer"], hp["falcon_type"],
                                    n_ctx, n_batch, lf, ll, rank, world)
         self.layer_first, self.layer_last, self.rank, self.world = lf, ll, rank, world
-        self.h = self.L.b200_falcon_create(C.byref(self.params))
+        self.h = self.L.b200_falcon_create_kv(C.byref(self.params), 1 if kv_f16 else 0)
         self.n_vocab = hp["n_vocab"]
 
     @staticmethod
@@ -456,6 +461,14 @@ class Falcon:
         if n < 0:
             raise RuntimeError("b200_falcon_load_kv: missing / truncated / mismatching session file")
         return n
+
+    def kv_type(self):
+        """-> 0 (f32 cache) or 1 (fp16 cache)"""
+        return self.L.b200_falcon_kv_type(self.h)
+
+    def kv_device_bytes(self):
+        """-> device bytes of the KV cache plus its fp16 copies, all local layers"""
+        return self.L.b200_falcon_kv_device_bytes(self.h)
 
     def kv_fill_random(self, pos, n, seed=1):
         if self.L.b200_falcon_kv_fill_random(self.h, pos, n, seed) != 0:

@@ -13,6 +13,10 @@
 //     no [key][head] array, no shuffles; the scores travel through the same ring as the V rows
 // Against the oracle the tiny-model evals stay at the 1e-8 * S level.  Short contexts gain nothing; the decode graphs of engine.cu are
 // captured per tier.
+// An fp16 cache (template parameter E = __half) is already an exact mma operand: K and V rows go into the B fragments as they are, the
+// split falls away on the cache side -- scores Q_hi K + Q_lo K (2 mma instead of 3), values e V (1 mma instead of 2).  Nothing is
+// dropped beyond what the fp32 cache's split drops already (its lo x lo term), so the error bound of the tier is unchanged.
+#include <type_traits>
 #include "attn_split.cuh"
 
 __device__ __forceinline__ void cp_async16(void * smem, const void * g) { asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"(smem_u32(smem)), "l"(g) : "memory"); }
@@ -45,16 +49,25 @@ __device__ __forceinline__ void mma_1688(float (&d)[4], uint32_t a0, uint32_t a1
 }
 #define AL_KB 8                          // keys per warp and ring stage = the N of one mma
 #define AL_KR 2                          // ring stages per warp (double buffer)
-#define AL_KS 72                         // floats per K row in the ring: 64 + 8 keeps the B-fragment LDS.64s of a half-warp on distinct banks
-#define AL_VS 68                         // floats per V row in the ring: 64 + 4 does the same for the LDS.32s of the second product
+// Ring row strides in elements.  f32: K 64 + 8 keeps the B-fragment LDS.64s of a half-warp on distinct banks, V 64 + 4 does the same for
+// the LDS.32s of the second product.  fp16 (128-byte rows): K 64 + 8 puts the 32-bit word (gid, 8 t + tig) of a lane on bank
+// 4 gid + tig + 8 t -- 32 distinct banks; V 64 + 8 puts the 16-bit loads (keys 2 tig (+1), dim 8 nt + gid) on banks 8 tig + gid / 2
+// (+ 4), distinct per tig, lanes gid = 2 m, 2 m + 1 sharing a word; and 144-byte rows keep the 16-byte cp.async destinations aligned.
+template <typename E> struct AlRing;
+template <> struct AlRing<float>  { static constexpr int KS = 72, VS = 68; using E2 = float2; };
+template <> struct AlRing<__half> { static constexpr int KS = 72, VS = 72; using E2 = __half2; };
+__device__ __forceinline__ float al_cvt(float x, float *) { return x; }
+__device__ __forceinline__ __half al_cvt(float x, __half *) { return __float2half_rn(x); }
 // 8-key blocks of a split go round-robin to the warps: block b = stage * SPLIT_WARPS + warp
 __device__ __forceinline__ int warp_blocks(int nk, int warp) { const int nb = (nk + AL_KB - 1) / AL_KB; return nb > warp ? (nb - warp + SPLIT_WARPS - 1) / SPLIT_WARPS : 0; }
 
+template <typename E>
 __global__ void __launch_bounds__(SPLIT_THREADS, 4) attn_long_scores_kernel(const SplitArgs a) {
+    constexpr int KS = AlRing<E>::KS, CP = 16 / sizeof(E);                     // CP: elements per 16-byte copy
     __shared__ float wmax[SPLIT_WARPS][SPLIT_G];
-    __shared__ __align__(16) float ring[SPLIT_WARPS][AL_KR][AL_KB][AL_KS];    // 18 KB: K rows in flight
+    __shared__ __align__(16) E ring[SPLIT_WARPS][AL_KR][AL_KB][KS];           // 18 KB (f32) / 9 KB (fp16): K rows in flight
     __shared__ __align__(16) float qs[SPLIT_G][64];                           // this position's query rows, rotated
-    __shared__ __align__(16) float knew_s[AL_KS];                          // this position's key row, rotated (not in the cache yet)
+    __shared__ __align__(16) E knew_s[KS];                                    // this position's key row, rotated (not in the cache yet), as the cache holds it
     trace_begin(a.trace);
     const int split = blockIdx.x, kvh = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int h0 = kvh * a.G + blockIdx.z * SPLIT_G, G = min(SPLIT_G, a.G - (int) blockIdx.z * SPLIT_G);      // this CTA's query heads: h0 .. h0 + G - 1
@@ -78,15 +91,15 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 4) attn_long_scores_kernel(cons
     const int j_new = a.fuse_rope ? n_past - k_lo : -1;           // this position's key is not in the cache yet (another CTA may be writing it right now)
     const size_t kv_row = (size_t) a.n_head_kv * 64;
     const int gid = lane >> 2, tig = lane & 3;
-    const float * kp = a.kc + (size_t) kvh * 64 + 16 * tig + (size_t) k_lo * kv_row;
-    auto issue = [&](int i) {                                     // lane copies 64 bytes: dims 16 tig .. 16 tig + 15 of key gid of the block
+    const E * kp = split_cache<E>(a.kc) + (size_t) kvh * 64 + 16 * tig + (size_t) k_lo * kv_row;
+    auto issue = [&](int i) {                                     // lane copies dims 16 tig .. 16 tig + 15 of key gid of the block
         if (i < nst) {
             const int jj = (i * SPLIT_WARPS + warp) * AL_KB + gid;
             if (jj < nk && jj != j_new) {
-                float * dst = &ring[warp][i % AL_KR][gid][16 * tig];
-                const float * src = kp + (size_t) jj * kv_row;
+                E * dst = &ring[warp][i % AL_KR][gid][16 * tig];
+                const E * src = kp + (size_t) jj * kv_row;
 #pragma unroll
-                for (int c = 0; c < 4; c++) cp_async16(dst + 4 * c, src + 4 * c);
+                for (int c = 0; c < 16 / CP; c++) cp_async16(dst + CP * c, src + CP * c);
             }
         }
         cp_async_commit();
@@ -112,18 +125,13 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 4) attn_long_scores_kernel(cons
         }
         if (a.fuse_rope && warp == 0) {
             float y0, y1; rot(ka, kb_, y0, y1);
-            knew_s[ri] = y0; knew_s[ri + 32] = y1;
+            knew_s[ri] = al_cvt(y0, (E *) nullptr); knew_s[ri + 32] = al_cvt(y1, (E *) nullptr);
             if (blockIdx.z == 0 && n_past >= k_lo && n_past < k_hi) {                                                  // one warp appends K and V to the cache
                 const size_t o = ((size_t) n_past * a.n_head_kv + kvh) * 64;
                 const float * vsrc = a.qkv + (size_t) (a.n_head + a.n_head_kv + kvh) * 64;
                 const float v0 = vsrc[ri], v1 = vsrc[ri + 32];
-                a.kc_w[o + ri] = y0; a.kc_w[o + ri + 32] = y1;
-                a.vc_w[o + ri] = v0; a.vc_w[o + ri + 32] = v1;
-                if (a.k16) {
-                    a.k16[o + ri] = __float2half_rn(y0); a.k16[o + ri + 32] = __float2half_rn(y1);
-                    __half * vt = a.vt16 + (size_t) kvh * 64 * a.ctx_pad + n_past;
-                    vt[(size_t) ri * a.ctx_pad] = __float2half_rn(v0); vt[(size_t) (ri + 32) * a.ctx_pad] = __float2half_rn(v1);
-                }
+                kv_put_k(a.kc_w, a.k16, o + ri, y0); kv_put_k(a.kc_w, a.k16, o + ri + 32, y1);
+                kv_put_v(a.vc_w, a.v16, a.vt16, o + ri, kvh, ri, n_past, a.ctx_pad, v0); kv_put_v(a.vc_w, a.v16, a.vt16, o + ri + 32, kvh, ri + 32, n_past, a.ctx_pad, v1);
             }
         }
     }
@@ -144,14 +152,19 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 4) attn_long_scores_kernel(cons
         cp_async_wait<AL_KR - 1>();
         __syncwarp();                                             // the four lanes of a key copied a quarter of its row each
         const int jj0 = (i * SPLIT_WARPS + warp) * AL_KB;
-        const float * krow = jj0 + gid == j_new ? knew_s : &ring[warp][i % AL_KR][gid][0];     // B column gid = key jj0 + gid
+        const E * krow = jj0 + gid == j_new ? knew_s : &ring[warp][i % AL_KR][gid][0];     // B column gid = key jj0 + gid
         float c[4] = { 0.f, 0.f, 0.f, 0.f };
 #pragma unroll
         for (int t = 0; t < 4; t++) {
-            const float2 p0 = *reinterpret_cast<const float2 *>(krow + 16 * t + 2 * tig), p1 = *reinterpret_cast<const float2 *>(krow + 16 * t + 2 * tig + 8);
-            uint32_t bh0, bl0, bh1, bl1;
-            split_h2(p0.x, p0.y, bh0, bl0); split_h2(p1.x, p1.y, bh1, bl1);
-            mma_16816(c, ah[t], bh0, bh1); mma_16816(c, ah[t], bl0, bl1); mma_16816(c, al[t], bh0, bh1);
+            if constexpr (std::is_same<E, float>::value) {
+                const float2 p0 = *reinterpret_cast<const float2 *>(krow + 16 * t + 2 * tig), p1 = *reinterpret_cast<const float2 *>(krow + 16 * t + 2 * tig + 8);
+                uint32_t bh0, bl0, bh1, bl1;
+                split_h2(p0.x, p0.y, bh0, bl0); split_h2(p1.x, p1.y, bh1, bl1);
+                mma_16816(c, ah[t], bh0, bh1); mma_16816(c, ah[t], bl0, bl1); mma_16816(c, al[t], bh0, bh1);
+            } else {
+                const uint32_t b0 = *reinterpret_cast<const uint32_t *>(krow + 16 * t + 2 * tig), b1 = *reinterpret_cast<const uint32_t *>(krow + 16 * t + 2 * tig + 8);
+                mma_16816(c, ah[t], b0, b1); mma_16816(c, al[t], b0, b1);
+            }
         }
         // c0, c1: head gid, keys jj0 + 2 tig, + 1;  c2, c3: head gid + 8.  A key past the split's end had an unwritten ring row: its column is not stored
 #pragma unroll
@@ -179,13 +192,16 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 4) attn_long_scores_kernel(cons
     trace_end(a.trace);
 }
 
+template <typename E>
 __global__ void __launch_bounds__(SPLIT_THREADS, 4) attn_long_values_kernel(const SplitArgs a) {
-    // V rows in flight; once a warp has consumed its rows the same memory holds its partial outputs [head][64]
-    __shared__ __align__(16) float2 vring[SPLIT_WARPS][AL_KR * AL_KB * AL_VS / 2];
+    constexpr int VS = AlRing<E>::VS, CP = 16 / sizeof(E);
+    using E2 = typename AlRing<E>::E2;
+    // V rows in flight; once a warp has consumed its rows the same memory holds its partial outputs [head][64] (sized for the larger use)
+    constexpr int RING2 = AL_KR * AL_KB * VS * (int) sizeof(E) / 8, WS = RING2 > SPLIT_G * 32 ? RING2 : SPLIT_G * 32;
+    __shared__ __align__(16) float2 vring[SPLIT_WARPS][WS];
     __shared__ float sring[SPLIT_WARPS][AL_KR][32][4];                // the scores of those rows, lane-private: (gid, 2 tig), (gid, 2 tig + 1), (gid + 8, ..)
     __shared__ float gmax[SPLIT_G];
     __shared__ double dsum[SPLIT_WARPS][SPLIT_G];
-    static_assert(AL_KR * AL_KB * AL_VS / 2 >= SPLIT_G * 32, "a warp's ring doubles as its [SPLIT_G][64] partial-output block");
     const int split = blockIdx.x, kvh = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int h0 = kvh * a.G + blockIdx.z * SPLIT_G, G = min(SPLIT_G, a.G - (int) blockIdx.z * SPLIT_G);
     const int n_past = a.n_past_dev ? *a.n_past_dev : a.n_past, T = n_past + 1;
@@ -196,22 +212,22 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 4) attn_long_values_kernel(cons
     const int n_used = splits_used(T, a.n_splits);                // splits 0 .. n_used - 1 hold keys
     const int j_new = n_past - k_lo;                              // this position's V row is appended by the scores kernel: read after the wait
     const int gid = lane >> 2, tig = lane & 3;
-    const float * vp = a.vc + (size_t) kvh * 64 + 16 * tig + (size_t) k_lo * kv_row;
+    const E * vp = split_cache<E>(a.vc) + (size_t) kvh * 64 + 16 * tig + (size_t) k_lo * kv_row;
     const float * S0 = a.S + (size_t) (h0 + min(gid, G - 1)) * a.n_ctx + k_lo, * S1 = a.S + (size_t) (h0 + min(gid + 8, G - 1)) * a.n_ctx + k_lo;
-    float (*vr)[AL_KB][AL_VS] = reinterpret_cast<float (*)[AL_KB][AL_VS]>(vring[warp]);
+    E (*vr)[AL_KB][VS] = reinterpret_cast<E (*)[AL_KB][VS]>(vring[warp]);
     auto issue = [&](int i, bool v, bool s) {
         if (i < nst) {
             const int jj0 = (i * SPLIT_WARPS + warp) * AL_KB;
-            if (v) {                                              // lane copies 64 bytes: dims 16 tig .. + 15 of key gid; rows past the end are zeroed (0 x garbage could be NaN)
+            if (v) {                                              // lane copies dims 16 tig .. + 15 of key gid; rows past the end are zeroed (0 x garbage could be NaN)
                 const int jj = jj0 + gid;
-                float * dst = &vr[i % AL_KR][gid][16 * tig];
+                E * dst = &vr[i % AL_KR][gid][16 * tig];
                 if (jj < nk && jj != j_new) {
-                    const float * src = vp + (size_t) jj * kv_row;
+                    const E * src = vp + (size_t) jj * kv_row;
 #pragma unroll
-                    for (int c = 0; c < 4; c++) cp_async16(dst + 4 * c, src + 4 * c);
+                    for (int c = 0; c < 16 / CP; c++) cp_async16(dst + CP * c, src + CP * c);
                 } else if (jj >= nk) {
 #pragma unroll
-                    for (int c = 0; c < 4; c++) *reinterpret_cast<float4 *>(dst + 4 * c) = make_float4(0.f, 0.f, 0.f, 0.f);
+                    for (int c = 0; c < 16 / CP; c++) *reinterpret_cast<float4 *>(dst + CP * c) = make_float4(0.f, 0.f, 0.f, 0.f);
                 }
             }
             if (s) {
@@ -232,7 +248,8 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 4) attn_long_values_kernel(cons
 #pragma unroll
     for (int i = 0; i < AL_KR - 1; i++) issue(i, false, true);    // their scores, together with the split maxima: one round trip
     const bool has_new = j_new >= 0 && j_new < nk;
-    const float2 vnew = has_new ? *reinterpret_cast<const float2 *>(a.vc + (size_t) kvh * 64 + 2 * lane + (size_t) (k_lo + j_new) * kv_row) : make_float2(0.f, 0.f);
+    E2 vnew{};
+    if (has_new) vnew = *reinterpret_cast<const E2 *>(split_cache<E>(a.vc) + (size_t) kvh * 64 + 2 * lane + (size_t) (k_lo + j_new) * kv_row);
     if (tid < SPLIT_G) {
         float mx = -INFINITY;
         if (tid < G) for (int s = 0; s < n_used; s++) mx = fmaxf(mx, a.pmax[(size_t) (h0 + tid) * SPLIT_MAX + s]);
@@ -251,7 +268,7 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 4) attn_long_values_kernel(cons
         __syncwarp();
         const int jj0 = (i * SPLIT_WARPS + warp) * AL_KB, st = i % AL_KR;
         if (has_new && j_new >= jj0 && j_new < jj0 + AL_KB) {     // this position's V row goes into its ring row now
-            *reinterpret_cast<float2 *>(&vr[st][j_new - jj0][2 * lane]) = vnew;
+            *reinterpret_cast<E2 *>(&vr[st][j_new - jj0][2 * lane]) = vnew;
             __syncwarp();
         }
         // e = table_exp_f16[f16(s - max)] (ggml.c:12427-12440), produced directly in A-fragment layout: a0 = (gid; keys 2 tig, + 1), a1 = (gid + 8; ..)
@@ -267,9 +284,14 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 4) attn_long_values_kernel(cons
         const uint32_t a0 = *reinterpret_cast<const uint32_t *>(&e0h), a1 = *reinterpret_cast<const uint32_t *>(&e1h);
 #pragma unroll
         for (int nt = 0; nt < 8; nt++) {                                         // B column gid = dim 8 nt + gid, rows = keys 2 tig, 2 tig + 1
-            uint32_t bh, bl;
-            split_h2(vr[st][2 * tig][8 * nt + gid], vr[st][2 * tig + 1][8 * nt + gid], bh, bl);
-            mma_1688(acc[nt], a0, a1, bh); mma_1688(acc[nt], a0, a1, bl);
+            if constexpr (std::is_same<E, float>::value) {
+                uint32_t bh, bl;
+                split_h2(vr[st][2 * tig][8 * nt + gid], vr[st][2 * tig + 1][8 * nt + gid], bh, bl);
+                mma_1688(acc[nt], a0, a1, bh); mma_1688(acc[nt], a0, a1, bl);
+            } else {
+                const __half2 b = __halves2half2(vr[st][2 * tig][8 * nt + gid], vr[st][2 * tig + 1][8 * nt + gid]);
+                mma_1688(acc[nt], a0, a1, *reinterpret_cast<const uint32_t *>(&b));
+            }
         }
         __syncwarp();                                             // all reads of this stage are done before the next iteration refills it
     }
@@ -300,10 +322,12 @@ void launch_attention_long(SplitArgs a, cudaStream_t stream) {
     a.n_splits = a.n_splits < 4 ? 4 : a.n_splits > SPLIT_MAX ? SPLIT_MAX : a.n_splits;
     static bool set = false;
     if (!set) {
-        B200_CUDA_CHECK(cudaFuncSetAttribute(attn_long_scores_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, B200_CARVEOUT));
-        B200_CUDA_CHECK(cudaFuncSetAttribute(attn_long_values_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, B200_CARVEOUT));
+        for (const void * k : { (const void *) attn_long_scores_kernel<float>, (const void *) attn_long_values_kernel<float>,
+                                (const void *) attn_long_scores_kernel<__half>, (const void *) attn_long_values_kernel<__half> })
+            B200_CUDA_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, B200_CARVEOUT));
         set = true;
     }
     g_long_launches++;
-    split_launch(attn_long_scores_kernel, attn_long_values_kernel, a, 0, stream);
+    if (a.kv16) split_launch(attn_long_scores_kernel<__half>, attn_long_values_kernel<__half>, a, 0, stream);
+    else split_launch(attn_long_scores_kernel<float>, attn_long_values_kernel<float>, a, 0, stream);
 }

@@ -231,16 +231,17 @@ PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
     return fn;
 }
 
-// fp32 cache rows [pos, pos + n) -> the fp16 shadows (used when a cache was filled by something other than rope_kv_append:
-// session restore, the per-operator C ABI)
-__global__ void kv_shadow_refresh_kernel(const float * __restrict__ kc, const float * __restrict__ vc, __half * __restrict__ k16, __half * __restrict__ vt16,
+// cache rows [pos, pos + n) -> the fp16 planes the prompt kernel reads (used when a cache was filled by something other than
+// rope_kv_append: session restore, kv_write, the per-operator C ABI).  fp32 cache: k16 and vt16; fp16 cache (T = __half): vt16 only
+template <typename T>
+__global__ void kv_shadow_refresh_kernel(const T * __restrict__ kc, const T * __restrict__ vc, __half * __restrict__ k16, __half * __restrict__ vt16,
                                          int n_head_kv, int ctx_pad, int pos, int n) {
     const int64_t total = (int64_t) n * n_head_kv * 64;
     for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t) gridDim.x * blockDim.x) {
         const int d = (int) (i % 64), h = (int) ((i / 64) % n_head_kv), p = pos + (int) (i / (64 * n_head_kv));
         const size_t src = ((size_t) p * n_head_kv + h) * 64 + d;
-        k16[src] = __float2half_rn(kc[src]);
-        vt16[((size_t) h * 64 + d) * ctx_pad + p] = __float2half_rn(vc[src]);
+        if (kc) k16[src] = __float2half_rn(kv_ld(kc + src));
+        vt16[((size_t) h * 64 + d) * ctx_pad + p] = __float2half_rn(kv_ld(vc + src));
     }
 }
 
@@ -256,6 +257,13 @@ void launch_kv_shadow_refresh(const float * k_cache, const float * v_cache, __ha
     const int64_t total = (int64_t) n * n_head_kv * 64;
     const unsigned grid = (unsigned) (total / 256 + 1 > 132 * 8 ? 132 * 8 : total / 256 + 1);
     kv_shadow_refresh_kernel<<<grid, 256, 0, stream>>>(k_cache, v_cache, k16, vt16, n_head_kv, attention_ctx_pad(n_ctx), pos, n);
+    B200_CUDA_CHECK(cudaGetLastError());
+}
+void launch_kv_shadow_refresh(const __half * v16, __half * vt16, int n_head_kv, int n_ctx, int pos, int n, cudaStream_t stream) {
+    if (n <= 0) return;
+    const int64_t total = (int64_t) n * n_head_kv * 64;
+    const unsigned grid = (unsigned) (total / 256 + 1 > 132 * 8 ? 132 * 8 : total / 256 + 1);
+    kv_shadow_refresh_kernel<__half><<<grid, 256, 0, stream>>>(nullptr, v16, nullptr, vt16, n_head_kv, attention_ctx_pad(n_ctx), pos, n);
     B200_CUDA_CHECK(cudaGetLastError());
 }
 

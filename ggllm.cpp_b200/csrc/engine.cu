@@ -69,8 +69,10 @@ struct b200_falcon {
     std::vector<Layer> layers;
     WPlanes tok_emb{}, lm_head{};
     float * lnf_g = nullptr, * lnf_b = nullptr;
-    float * k_cache = nullptr, * v_cache = nullptr;
-    __half * k16 = nullptr, * vt16 = nullptr; size_t shadow_layer = 0;      // fp16 shadow of the cache for the prompt kernel (attention_ws.cu); only when n_batch > 8
+    int kv_type = T_F32;                        // the cache's element type: T_F32, or T_F16 (b200_falcon_create_kv)
+    float * k_cache = nullptr, * v_cache = nullptr;                        // f32 cache (null in an fp16 engine)
+    __half * k16 = nullptr, * vt16 = nullptr; size_t shadow_layer = 0;      // fp16 K plane for the prompt kernel (attention_ws.cu) -- the K cache itself in an fp16 engine -- and V^T (only when n_batch > 8); shadow_layer: halves per layer of each plane
+    __half * v16 = nullptr;                                                // fp16 engine: the V cache
     // activation arena
     float * inp = nullptr, * qkv = nullptr, * att = nullptr, * ao = nullptr, * up = nullptr, * dn = nullptr, * logits = nullptr;
     void * actq_mem = nullptr; ActQ xa{}, xm{}, xatt{}, xup{}, xf{};
@@ -110,21 +112,27 @@ struct b200_falcon {
                  std::vector<int> rotated; } tap;                // rotated[l]: RoPE ran in place on qkv (not inside the attention kernels)
 };
 
-// Local layer l's slice of the KV cache.  k / v: [n_ctx][n_head_kv][head_dim] f32, rows of kv_row() floats.  k16 / vt16: its fp16
-// shadow in the layout of AttnParams::k16 / vt16, null when the engine keeps none.
-struct KvLayer { float * k, * v; __half * k16, * vt16; };
+// Local layer l's slice of the KV cache.  f32 engine: k / v [n_ctx][n_head_kv][head_dim] f32, rows of kv_row() floats, and k16 / vt16 its
+// fp16 shadow in the layout of AttnParams::k16 / vt16 (null when the engine keeps none).  fp16 engine: k16 / v16 [n_ctx][n_head_kv][head_dim]
+// are the cache (k / v null), vt16 as above.
+struct KvLayer { float * k, * v; __half * k16, * vt16, * v16; };
 static size_t kv_row(const b200_falcon * f) { return (size_t) f->HKV * f->D; }
 static KvLayer kv_layer(const b200_falcon * f, int l) {
-    const size_t off = (size_t) l * f->hp.n_ctx * kv_row(f);
-    KvLayer c = { f->k_cache + off, f->v_cache + off, nullptr, nullptr };
-    if (f->k16) { c.k16 = f->k16 + (size_t) l * f->shadow_layer; c.vt16 = f->vt16 + (size_t) l * f->shadow_layer; }
+    KvLayer c = { nullptr, nullptr, nullptr, nullptr, nullptr };
+    const size_t off = (size_t) l * f->hp.n_ctx * kv_row(f), off16 = (size_t) l * f->shadow_layer;
+    if (f->k_cache) { c.k = f->k_cache + off; c.v = f->v_cache + off; }
+    if (f->k16) c.k16 = f->k16 + off16;
+    if (f->vt16) c.vt16 = f->vt16 + off16;
+    if (f->v16) c.v16 = f->v16 + off16;
     return c;
 }
 
-__global__ void fill_f32_kernel(float * p, int64_t n, float base, float amp, uint64_t seed) {
+template <typename E>
+__global__ void fill_kernel(E * p, int64_t n, float base, float amp, uint64_t seed) {
     for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x * blockDim.x) {
         uint64_t x = seed + (uint64_t) i * 0x9E3779B97F4A7C15ULL; x ^= x >> 31; x *= 0xBF58476D1CE4E5B9ULL; x ^= x >> 29;
-        p[i] = base + amp * ((float) (x & 0xffffff) / 8388608.f - 1.f);
+        const float v = base + amp * ((float) (x & 0xffffff) / 8388608.f - 1.f);
+        if constexpr (sizeof(E) == 2) p[i] = __float2half_rn(v); else p[i] = v;
     }
 }
 
@@ -229,9 +237,12 @@ static void classify(b200_falcon * f) {
 
 extern "C" {
 
-b200_falcon * b200_falcon_create(const b200_falcon_params * p) {
+b200_falcon * b200_falcon_create(const b200_falcon_params * p) { return b200_falcon_create_kv(p, T_F32); }
+b200_falcon * b200_falcon_create_kv(const b200_falcon_params * p, int kv_ggml_type) {
+    if (kv_ggml_type != T_F32 && kv_ggml_type != T_F16) return nullptr;
     b200_falcon * f = new b200_falcon();
     f->hp = *p;
+    f->kv_type = kv_ggml_type;
     B200_ASSERT(p->n_embd % p->n_head == 0 && p->n_head % p->n_head_kv == 0);
     f->E = p->n_embd; f->H = p->n_head; f->HKV = p->n_head_kv; f->D = p->n_embd / p->n_head;
     f->QKV = (f->H + 2 * f->HKV) * f->D; f->FF = 4 * f->E; f->V = p->n_vocab;
@@ -246,14 +257,20 @@ b200_falcon * b200_falcon_create(const b200_falcon_params * p) {
     B200_CUDA_CHECK(cudaEventCreateWithFlags(&f->e_join, cudaEventDisableTiming));
     B200_CUDA_CHECK(cudaEventCreate(&f->e_t0)); B200_CUDA_CHECK(cudaEventCreate(&f->e_t1));
     const size_t NB = (size_t) (p->n_batch > 0 ? p->n_batch : 1);
-    const size_t kv = (size_t) f->NL * p->n_ctx * kv_row(f) * sizeof(float);
-    B200_CUDA_CHECK(cudaMalloc(&f->k_cache, kv ? kv : 4)); B200_CUDA_CHECK(cudaMalloc(&f->v_cache, kv ? kv : 4));
-    B200_CUDA_CHECK(cudaMemset(f->k_cache, 0, kv)); B200_CUDA_CHECK(cudaMemset(f->v_cache, 0, kv));
-    if (p->n_batch > b200_mmv_max_n() && f->D == 64 && f->NL > 0) {
-        f->shadow_layer = attention_shadow_halves(f->HKV, p->n_ctx);
+    const bool shadow = p->n_batch > b200_mmv_max_n() && f->D == 64 && f->NL > 0;      // the prompt kernel's fp16 planes
+    auto alloc16 = [&](__half ** d) {
         const size_t sb = (size_t) f->NL * f->shadow_layer * sizeof(__half);
-        B200_CUDA_CHECK(cudaMalloc(&f->k16, sb)); B200_CUDA_CHECK(cudaMalloc(&f->vt16, sb));
-        B200_CUDA_CHECK(cudaMemset(f->k16, 0, sb)); B200_CUDA_CHECK(cudaMemset(f->vt16, 0, sb));
+        B200_CUDA_CHECK(cudaMalloc(d, sb ? sb : 4)); B200_CUDA_CHECK(cudaMemset(*d, 0, sb));
+    };
+    if (f->kv_type == T_F16) {                   // the cache is the fp16 K plane and V rows (rows padded to a multiple of 64 like the planes)
+        f->shadow_layer = (size_t) attention_ctx_pad(p->n_ctx) * kv_row(f);
+        alloc16(&f->k16); alloc16(&f->v16);
+        if (shadow) alloc16(&f->vt16);
+    } else {
+        const size_t kv = (size_t) f->NL * p->n_ctx * kv_row(f) * sizeof(float);
+        B200_CUDA_CHECK(cudaMalloc(&f->k_cache, kv ? kv : 4)); B200_CUDA_CHECK(cudaMalloc(&f->v_cache, kv ? kv : 4));
+        B200_CUDA_CHECK(cudaMemset(f->k_cache, 0, kv)); B200_CUDA_CHECK(cudaMemset(f->v_cache, 0, kv));
+        if (shadow) { f->shadow_layer = attention_shadow_halves(f->HKV, p->n_ctx); alloc16(&f->k16); alloc16(&f->vt16); }
     }
     B200_CUDA_CHECK(cudaMalloc(&f->inp, NB * f->E * 4)); B200_CUDA_CHECK(cudaMalloc(&f->qkv, NB * f->QKV * 4));
     B200_CUDA_CHECK(cudaMalloc(&f->att, NB * f->E * 4)); B200_CUDA_CHECK(cudaMalloc(&f->ao, NB * f->E * 4));
@@ -343,7 +360,7 @@ static void place_tensor(b200_falcon * f, const Slot & s, int type, const void *
         B200_CUDA_CHECK(cudaMalloc(&v, (size_t) K * 4));
         if (random) {                               // LayerNorm gamma around 1, beta around 0
             const bool gamma = s.d->kind == S_LNF_G || s.d->kind == S_LN_ATTN_G || s.d->kind == S_LN_MLP_G;
-            fill_f32_kernel<<<32, 256, 0, st>>>(v, K, gamma ? 1.f : 0.f, gamma ? 0.1f : 0.01f, seed); B200_CUDA_CHECK(cudaGetLastError());
+            fill_kernel<<<32, 256, 0, st>>>(v, K, gamma ? 1.f : 0.f, gamma ? 0.1f : 0.01f, seed); B200_CUDA_CHECK(cudaGetLastError());
         } else {
             B200_ASSERT(type == T_F32);
             B200_CUDA_CHECK(cudaMemcpyAsync(v, host_data, (size_t) K * 4, cudaMemcpyHostToDevice, st));
@@ -499,7 +516,7 @@ void b200_falcon_free(b200_falcon * f) {
     for (auto & L : f->layers) { free_matrix(f, L.wqkv); free_matrix(f, L.wo); free_matrix(f, L.up); free_matrix(f, L.down);
         cudaFree(L.ln_attn_g); cudaFree(L.ln_attn_b); cudaFree(L.ln_mlp_g); cudaFree(L.ln_mlp_b); }
     free_matrix(f, f->tok_emb); free_matrix(f, f->lm_head);
-    cudaFree(f->lnf_g); cudaFree(f->lnf_b); cudaFree(f->k_cache); cudaFree(f->v_cache); cudaFree(f->k16); cudaFree(f->vt16);
+    cudaFree(f->lnf_g); cudaFree(f->lnf_b); cudaFree(f->k_cache); cudaFree(f->v_cache); cudaFree(f->k16); cudaFree(f->vt16); cudaFree(f->v16);
     cudaFree(f->inp); cudaFree(f->qkv); cudaFree(f->att); cudaFree(f->ao); cudaFree(f->up); cudaFree(f->dn); cudaFree(f->logits);
     cudaFree(f->attn_scratch); cudaFree(f->actq_mem); cudaFree(f->gen_na); cudaFree(f->gen_nm); cudaFree(f->gen_actq); cudaFree(f->gen_xh); cudaFree(f->xh_a); cudaFree(f->xh_b); cudaFree(f->xh_m);
     cudaFree(f->tokens_dev); cudaFree(f->n_past_dev); cudaFree(f->q_ctr); cudaFree(f->attn_dec_scratch); cudaFree(f->tap.mem);
@@ -622,7 +639,7 @@ static AttnParams attn_params(const b200_falcon * f, int l, int N, int n_past, f
     ap.long_ctx = graph_mode ? f->cur_tier : 0;
     ap.rope_theta_scale = theta_scale;
     const KvLayer kv = kv_layer(f, l);
-    ap.k16 = kv.k16; ap.vt16 = kv.vt16;
+    ap.k16 = kv.k16; ap.vt16 = kv.vt16; ap.v16 = kv.v16;
     return ap;
 }
 // RoPE + KV append of layer l's new rows (:2229-2281), then the attention qkv -> att (:2285-2366).  Prompts run eagerly, on s_main
@@ -947,21 +964,37 @@ static int generate_impl(b200_falcon * f, int32_t first_token, int n_past, int n
 }
 // ---- KV cache access (session state, SURVEY 8f-4).  The reference serialises its KV cache with the context
 // (falcon_copy_state_data / falcon_set_state_data, libfalcon.cpp:4313-4490: n_tokens x n_embd_kv floats per layer for K and V);
-// here the cache is device-resident [layer][n_ctx][n_head_kv][head_dim] f32 and rows are copied straight out of / into HBM.
+// here the cache is device-resident [layer][n_ctx][n_head_kv][head_dim] f32 or fp16 and rows are copied straight out of / into HBM.  The
+// host rows are f32 for either engine: an fp16 cache's values are widened exactly on the way out and rounded (to nearest even) on the way in.
+static void kv16_d2h(float * dst, const __half * src, size_t n) {
+    std::vector<__half> h(n);
+    B200_CUDA_CHECK(cudaMemcpy(h.data(), src, n * 2, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < n; i++) dst[i] = __half2float(h[i]);
+}
+static void kv16_h2d(__half * dst, const float * src, size_t n) {
+    std::vector<__half> h(n);
+    for (size_t i = 0; i < n; i++) h[i] = __float2half_rn(src[i]);
+    B200_CUDA_CHECK(cudaMemcpy(dst, h.data(), n * 2, cudaMemcpyHostToDevice));
+}
 int b200_falcon_kv_read(b200_falcon * f, int layer, int pos, int n, float * k_out, float * v_out) {
     if (layer < f->hp.layer_first || layer >= f->hp.layer_last || pos < 0 || n < 0 || pos + n > f->hp.n_ctx) return 1;
     const KvLayer c = kv_layer(f, layer - f->hp.layer_first);
-    const size_t row = kv_row(f);
+    const size_t row = kv_row(f), o = (size_t) pos * row, cnt = (size_t) n * row;
     B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
-    if (k_out) B200_CUDA_CHECK(cudaMemcpy(k_out, c.k + (size_t) pos * row, (size_t) n * row * 4, cudaMemcpyDeviceToHost));
-    if (v_out) B200_CUDA_CHECK(cudaMemcpy(v_out, c.v + (size_t) pos * row, (size_t) n * row * 4, cudaMemcpyDeviceToHost));
+    if (f->kv_type == T_F16) {
+        if (k_out) kv16_d2h(k_out, c.k16 + o, cnt);
+        if (v_out) kv16_d2h(v_out, c.v16 + o, cnt);
+        return 0;
+    }
+    if (k_out) B200_CUDA_CHECK(cudaMemcpy(k_out, c.k + o, cnt * 4, cudaMemcpyDeviceToHost));
+    if (v_out) B200_CUDA_CHECK(cudaMemcpy(v_out, c.v + o, cnt * 4, cudaMemcpyDeviceToHost));
     return 0;
 }
-// the fp16 shadow the prompt kernel reads (attention_ws.cu), positions [pos, pos + n) of `layer`: k16_out [n][n_head_kv][head_dim],
-// vt16_out [n_head_kv][head_dim][n].  The range may reach attention_ctx_pad(n_ctx), so that the padding columns can be inspected.
+// the fp16 planes the prompt kernel reads (attention_ws.cu), positions [pos, pos + n) of `layer`: k16_out [n][n_head_kv][head_dim] (an fp16
+// engine's K cache itself), vt16_out [n_head_kv][head_dim][n].  The range may reach attention_ctx_pad(n_ctx), so that the padding can be inspected.
 int b200_falcon_kv_shadow_read(b200_falcon * f, int layer, int pos, int n, uint16_t * k16_out, uint16_t * vt16_out) {
     const int ctx_pad = attention_ctx_pad(f->hp.n_ctx);
-    if (!f->k16 || layer < f->hp.layer_first || layer >= f->hp.layer_last || pos < 0 || n < 0 || pos + n > ctx_pad) return 1;
+    if (!f->k16 || (vt16_out && !f->vt16) || layer < f->hp.layer_first || layer >= f->hp.layer_last || pos < 0 || n < 0 || pos + n > ctx_pad) return 1;
     const KvLayer c = kv_layer(f, layer - f->hp.layer_first);
     const size_t row = kv_row(f);
     B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
@@ -972,14 +1005,18 @@ int b200_falcon_kv_shadow_read(b200_falcon * f, int layer, int pos, int n, uint1
 int b200_falcon_kv_write(b200_falcon * f, int layer, int pos, int n, const float * k_in, const float * v_in) {
     if (layer < f->hp.layer_first || layer >= f->hp.layer_last || pos < 0 || n < 0 || pos + n > f->hp.n_ctx) return 1;
     const KvLayer c = kv_layer(f, layer - f->hp.layer_first);
-    const size_t row = kv_row(f);
+    const size_t row = kv_row(f), o = (size_t) pos * row, cnt = (size_t) n * row;
     B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
-    if (k_in) B200_CUDA_CHECK(cudaMemcpy(c.k + (size_t) pos * row, k_in, (size_t) n * row * 4, cudaMemcpyHostToDevice));
-    if (v_in) B200_CUDA_CHECK(cudaMemcpy(c.v + (size_t) pos * row, v_in, (size_t) n * row * 4, cudaMemcpyHostToDevice));
-    if (c.k16) {
-        launch_kv_shadow_refresh(c.k, c.v, c.k16, c.vt16, f->HKV, f->hp.n_ctx, pos, n, f->s_main);
-        B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
+    if (f->kv_type == T_F16) {
+        if (k_in) kv16_h2d(c.k16 + o, k_in, cnt);
+        if (v_in) kv16_h2d(c.v16 + o, v_in, cnt);
+        if (c.vt16) launch_kv_shadow_refresh(c.v16, c.vt16, f->HKV, f->hp.n_ctx, pos, n, f->s_main);
+    } else {
+        if (k_in) B200_CUDA_CHECK(cudaMemcpy(c.k + o, k_in, cnt * 4, cudaMemcpyHostToDevice));
+        if (v_in) B200_CUDA_CHECK(cudaMemcpy(c.v + o, v_in, cnt * 4, cudaMemcpyHostToDevice));
+        if (c.k16) launch_kv_shadow_refresh(c.k, c.v, c.k16, c.vt16, f->HKV, f->hp.n_ctx, pos, n, f->s_main);
     }
+    B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
     return 0;
 }
 // random K / V rows generated on the device for positions [pos, pos + n) of every local layer: pre-fills a long context
@@ -989,8 +1026,15 @@ int b200_falcon_kv_fill_random(b200_falcon * f, int pos, int n, uint64_t seed) {
     const size_t row = kv_row(f);
     for (int l = 0; l < f->NL; l++) {
         const KvLayer c = kv_layer(f, l);
-        fill_f32_kernel<<<296, 256, 0, f->s_main>>>(c.k + (size_t) pos * row, (int64_t) ((size_t) n * row), 0.f, 1.f, seed + 2 * l);
-        fill_f32_kernel<<<296, 256, 0, f->s_main>>>(c.v + (size_t) pos * row, (int64_t) ((size_t) n * row), 0.f, 1.f, seed + 2 * l + 1);
+        const int64_t cnt = (int64_t) ((size_t) n * row);
+        if (f->kv_type == T_F16) {                                   // the same values, rounded to the cache's fp16
+            fill_kernel<<<296, 256, 0, f->s_main>>>(c.k16 + (size_t) pos * row, cnt, 0.f, 1.f, seed + 2 * l);
+            fill_kernel<<<296, 256, 0, f->s_main>>>(c.v16 + (size_t) pos * row, cnt, 0.f, 1.f, seed + 2 * l + 1);
+            if (c.vt16) launch_kv_shadow_refresh(c.v16, c.vt16, f->HKV, f->hp.n_ctx, pos, n, f->s_main);
+            continue;
+        }
+        fill_kernel<<<296, 256, 0, f->s_main>>>(c.k + (size_t) pos * row, cnt, 0.f, 1.f, seed + 2 * l);
+        fill_kernel<<<296, 256, 0, f->s_main>>>(c.v + (size_t) pos * row, cnt, 0.f, 1.f, seed + 2 * l + 1);
         if (c.k16) launch_kv_shadow_refresh(c.k, c.v, c.k16, c.vt16, f->HKV, f->hp.n_ctx, pos, n, f->s_main);
     }
     B200_CUDA_CHECK(cudaGetLastError());
@@ -1001,6 +1045,7 @@ int b200_falcon_kv_fill_random(b200_falcon * f, int pos, int n, uint64_t seed) {
 // the KV state, written straight from / read straight into HBM through a bounded pinned buffer.  Own container (the reference's
 // serialises its transposed, ping-ponged host V buffers, which do not exist here):
 //   u32 magic 'b2kv', u32 version 1, i32 layer_first, layer_last, n_head_kv, head_dim, n_tokens; then per local layer: K rows, V rows (f32)
+// for either cache type (kv_read / kv_write: an fp16 engine's file round-trips bit for bit, an f32 file loaded into it is rounded)
 // save: returns 0 / -1.  load: returns the number of positions restored (the caller continues at that n_past), -1 on any mismatch.
 int b200_falcon_save_kv(b200_falcon * f, const char * path, int n_tokens) {
     if (n_tokens < 0 || n_tokens > f->hp.n_ctx) return -1;
@@ -1009,13 +1054,11 @@ int b200_falcon_save_kv(b200_falcon * f, const char * path, int n_tokens) {
     const int32_t hdr[7] = { 0x766b3262, 1, f->hp.layer_first, f->hp.layer_last, f->HKV, f->D, n_tokens };
     bool ok = fwrite(hdr, sizeof(hdr), 1, fp) == 1;
     const size_t bytes = (size_t) n_tokens * kv_row(f) * 4;
-    std::vector<float> buf(bytes / 4 + 1);
-    B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
-    for (int l = 0; l < f->NL && ok; l++)
-        for (const float * base : { kv_layer(f, l).k, kv_layer(f, l).v }) {
-            B200_CUDA_CHECK(cudaMemcpy(buf.data(), base, bytes, cudaMemcpyDeviceToHost));
-            ok = ok && (bytes == 0 || fwrite(buf.data(), bytes, 1, fp) == 1);
-        }
+    std::vector<float> k(bytes / 4 + 1), v(bytes / 4 + 1);
+    for (int l = 0; l < f->NL && ok; l++) {
+        b200_falcon_kv_read(f, f->hp.layer_first + l, 0, n_tokens, k.data(), v.data());
+        ok = bytes == 0 || (fwrite(k.data(), bytes, 1, fp) == 1 && fwrite(v.data(), bytes, 1, fp) == 1);
+    }
     ok = (fclose(fp) == 0) && ok;
     return ok ? 0 : -1;
 }
@@ -1030,7 +1073,7 @@ int b200_falcon_load_kv(b200_falcon * f, const char * path) {
     std::vector<float> k(bytes / 4 + 1), v(bytes / 4 + 1);
     for (int l = 0; l < f->NL; l++) {
         if (bytes && (fread(k.data(), bytes, 1, fp) != 1 || fread(v.data(), bytes, 1, fp) != 1)) { fclose(fp); return -1; }
-        if (b200_falcon_kv_write(f, f->hp.layer_first + l, 0, n, k.data(), v.data()) != 0) { fclose(fp); return -1; }     // also refreshes the fp16 shadow
+        if (b200_falcon_kv_write(f, f->hp.layer_first + l, 0, n, k.data(), v.data()) != 0) { fclose(fp); return -1; }     // also refreshes the fp16 planes
     }
     fclose(fp);
     return n;
@@ -1102,6 +1145,11 @@ int b200_falcon_tap_read(const b200_falcon * f, int layer, const char * node, vo
     return 1;
 }
 
+int b200_falcon_kv_type(const b200_falcon * f) { return f->kv_type; }
+size_t b200_falcon_kv_device_bytes(const b200_falcon * f) {
+    const size_t planes16 = (f->k16 ? 1 : 0) + (f->vt16 ? 1 : 0) + (f->v16 ? 1 : 0);
+    return (f->k_cache ? 2 * (size_t) f->NL * f->hp.n_ctx * kv_row(f) * sizeof(float) : 0) + planes16 * f->NL * f->shadow_layer * sizeof(__half);
+}
 int b200_falcon_last_launches(const b200_falcon * f) { return f->launches; }
 float b200_falcon_last_ms(const b200_falcon * f) { return f->last_ms; }
 void * b200_falcon_stream(b200_falcon * f) { return (void *) f->s_main; }

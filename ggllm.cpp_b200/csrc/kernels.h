@@ -70,7 +70,8 @@ struct AttnParams {
     unsigned long long * trace; // optional timeline slot (debug)
     const ActQ * qout;          // optional: also emit the output row quantised for the wo mat-mul (its INIT pass)
     // optional fp16 shadow of this layer's cache for the prompt kernel (attention_ws.cu): k16 [n_ctx][n_head_kv][64],
-    // vt16 [n_head_kv][64][attention_ctx_pad(n_ctx)] (V transposed); rope_kv_append keeps it in step with the fp32 cache
+    // vt16 [n_head_kv][64][attention_ctx_pad(n_ctx)] (V transposed); rope_kv_append keeps it in step with the fp32 cache.
+    // With an fp16 cache (v16 set) k16 IS the K cache and the fp32 cache pointers of the launchers are null.
     __half * k16; __half * vt16;
     // RoPE(Q, K) with rope_theta_scale and the KV append are part of launch_attention.  fuse_rope (decode): the split-KV scores kernel
     // may do them itself, on qkv's rows in registers, instead of a kernel of their own -- qkv is then NOT rotated in place.
@@ -79,7 +80,41 @@ struct AttnParams {
     // attention_long_threshold() keys, so the long-context kernels (attention_long.cu) may be captured; with a host n_past the launcher
     // decides by itself
     int long_ctx;
+    // fp16 KV cache (b200_falcon_create_kv with GGML_TYPE_F16): V rows [n_ctx][n_head_kv][head_dim] beside k16.  Rows are rounded to fp16
+    // when they are appended (__float2half_rn, ggml_fp32_to_fp16 on an F16C host) and every reader widens them exactly; null: fp32 cache
+    __half * v16;
 };
+static inline bool attn_kv16(const AttnParams & p) { return p.v16 != nullptr; }
+// The one writer of a cache element: every plane that exists gets it -- the fp32 row, the fp16 rows (k16 / v16), V^T (vt16, position
+// pos, dim d of KV head kvh).  An fp16 plane stores __float2half_rn(x): beyond +-65504 that is +-Inf.
+__device__ __forceinline__ void kv_put_k(float * kc, __half * k16, size_t o, float x) {
+    if (kc) kc[o] = x;
+    if (k16) k16[o] = __float2half_rn(x);
+}
+__device__ __forceinline__ void kv_put_v(float * vc, __half * v16, __half * vt16, size_t o, int kvh, int d, int pos, int ctx_pad, float x) {
+    if (vc) vc[o] = x;
+    if (v16) v16[o] = __float2half_rn(x);
+    if (vt16) vt16[((size_t) kvh * 64 + d) * ctx_pad + pos] = __float2half_rn(x);
+}
+// a cache element widened to f32 (exact for fp16)
+__device__ __forceinline__ float kv_ld(const float * p) { return *p; }
+__device__ __forceinline__ float kv_ld(const __half * p) { return __half2float(*p); }
+// two consecutive elements (8-byte / 4-byte aligned), read-only path
+__device__ __forceinline__ float2 kv_ld2(const float * p) { return __ldg(reinterpret_cast<const float2 *>(p)); }
+__device__ __forceinline__ float2 kv_ld2(const __half * p) { return __half22float2(__ldg(reinterpret_cast<const __half2 *>(p))); }
+// the same for a row the kernel in front of this one may just have written (not through the read-only path)
+__device__ __forceinline__ float2 kv_ld2_new(const float * p) { return *reinterpret_cast<const float2 *>(p); }
+__device__ __forceinline__ float2 kv_ld2_new(const __half * p) { return __half22float2(*reinterpret_cast<const __half2 *>(p)); }
+// elements 4 i .. 4 i + 3 of a row (16-byte / 8-byte aligned)
+__device__ __forceinline__ float4 kv_ld4(const float * p, int i) { return reinterpret_cast<const float4 *>(p)[i]; }
+__device__ __forceinline__ float4 kv_ld4(const __half * p, int i) {
+    const uint2 u = reinterpret_cast<const uint2 *>(p)[i];
+    const float2 a = __half22float2(*reinterpret_cast<const __half2 *>(&u.x)), b = __half22float2(*reinterpret_cast<const __half2 *>(&u.y));
+    return make_float4(a.x, a.y, b.x, b.y);
+}
+// what a reader of the cache sees of a value that has just been appended
+__device__ __forceinline__ float kv_seen(float x, const float *) { return x; }
+__device__ __forceinline__ float kv_seen(float x, const __half *) { return __half2float(__float2half_rn(x)); }
 // The attention scratch starts with this many bytes of split-KV arrival counters.  Their owner zeroes them once; they re-arm themselves.
 #define ATTN_CTR_BYTES 4096
 int    attention_long_threshold();          // keys above which decode attention switches to attention_long.cu
@@ -95,6 +130,7 @@ size_t attention_scratch_bytes(const AttnParams & p);                // one toke
 int    attention_ctx_pad(int n_ctx);
 size_t attention_shadow_halves(int n_head_kv, int n_ctx);           // halves per layer, for k16 and for vt16 each
 void   launch_kv_shadow_refresh(const float * k_cache, const float * v_cache, __half * k16, __half * vt16, int n_head_kv, int n_ctx, int pos, int n, cudaStream_t stream);
+void   launch_kv_shadow_refresh(const __half * v16, __half * vt16, int n_head_kv, int n_ctx, int pos, int n, cudaStream_t stream);   // fp16 cache: V^T only
 
 // ---- gemm.cu : Y[n][m] = sum_k W[m][k] * X[n][k], N large (prompt), wgmma tensor cores
 void   launch_mmq_gemm(const WPlanes & W, const __half * X, int64_t x_stride, int N, float * Y, int64_t y_stride, int epi_gelu, cudaStream_t stream);

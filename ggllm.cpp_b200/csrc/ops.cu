@@ -398,12 +398,11 @@ __global__ void rope_kv_append_kernel(float * __restrict__ qkv, float * __restri
     if (slot >= p.n_head) {
         const bool is_k = slot < p.n_head + p.n_head_kv;
         const int kvh = slot - p.n_head - (is_k ? 0 : p.n_head_kv);
-        float * dst = (is_k ? kc : vc) + ((size_t) pos * p.n_head_kv + kvh) * D;
-        dst[i] = v[i]; dst[i + half] = v[i + half];
-        if (p.k16) {                                                          // fp16 shadow for the prompt kernel, written once per token
-            if (is_k) { __half * d16 = p.k16 + ((size_t) pos * p.n_head_kv + kvh) * D; d16[i] = __float2half_rn(v[i]); d16[i + half] = __float2half_rn(v[i + half]); }
-            else { const size_t cp = (size_t) ((p.n_ctx + 63) / 64 * 64); __half * d16 = p.vt16 + (size_t) kvh * D * cp + pos;
-                   d16[(size_t) i * cp] = __float2half_rn(v[i]); d16[(size_t) (i + half) * cp] = __float2half_rn(v[i + half]); }
+        const size_t o = ((size_t) pos * p.n_head_kv + kvh) * D;
+        if (is_k) { kv_put_k(kc, p.k16, o + i, v[i]); kv_put_k(kc, p.k16, o + i + half, v[i + half]); }
+        else {
+            const int cp = (p.n_ctx + 63) / 64 * 64;
+            kv_put_v(vc, p.v16, p.vt16, o + i, kvh, i, pos, cp, v[i]); kv_put_v(vc, p.v16, p.vt16, o + i + half, kvh, i + half, pos, cp, v[i + half]);
         }
     }
     trace_end(p.trace);
@@ -432,12 +431,11 @@ __global__ void __launch_bounds__(256) rope_kv_append_batch_kernel(float * __res
             v[i] = r0; v[i + half] = r1;
             if (slot >= H) {
                 const size_t o = ((size_t) pos * HKV + (slot - H)) * D;
-                kc[o + i] = r0; kc[o + i + half] = r1;
-                if (p.k16) { p.k16[o + i] = __float2half_rn(r0); p.k16[o + i + half] = __float2half_rn(r1); }
+                kv_put_k(kc, p.k16, o + i, r0); kv_put_k(kc, p.k16, o + i + half, r1);
             }
         }
-        for (int idx = threadIdx.x; idx < HKV * D; idx += 256)
-            vc[(size_t) pos * HKV * D + idx] = row[(size_t) (H + HKV) * D + idx];
+        for (int idx = threadIdx.x; idx < HKV * D; idx += 256)         // V^T: the CTAs below
+            kv_put_v(vc, p.v16, nullptr, (size_t) pos * HKV * D + idx, 0, 0, 0, 0, row[(size_t) (H + HKV) * D + idx]);
     } else if (p.vt16) {
         __shared__ __half sm[64][66];
         const int tile = (int) blockIdx.x - N, tt = tile / HKV, kvh = tile % HKV;

@@ -139,6 +139,13 @@ void   b200_layernorm_q(float * x_dev, int64_t x_stride, const float * ra_dev, c
  * the wo mat-mul.  Returns 1 when that quantisation ran inside the attention combine step, 0 when it needed its own kernel. */
 int    b200_attention_decode(float * qkv_dev, float * k_cache_dev, float * v_cache_dev, float * out_dev,
                              int n_head, int n_head_kv, int head_dim, int n_past, int n_ctx, int n_ctx_rope, b200_actq * qout);
+/* test hooks: b200_attention / b200_attention_decode over an fp16 cache, k16 / v16 [n_ctx][n_head_kv][head_dim] fp16 bit patterns (row
+ * layout, what an engine made by b200_falcon_create_kv(.., GGML_TYPE_F16) holds).  The new rows are stored rounded to fp16, and every
+ * score and output reads the rounded values, the new token's own row included. */
+void   b200_attention_kv16(float * qkv_dev, uint16_t * k16_dev, uint16_t * v16_dev, float * out_dev, int n_head, int n_head_kv,
+                           int head_dim, int n_tok, int n_past, int n_ctx, int n_ctx_rope);
+int    b200_attention_decode_kv16(float * qkv_dev, uint16_t * k16_dev, uint16_t * v16_dev, float * out_dev, int n_head, int n_head_kv,
+                                  int head_dim, int n_past, int n_ctx, int n_ctx_rope, b200_actq * qout);
 
 /* ---- sampling on the device (SURVEY 8f-2): falcon_main's chain (examples/falcon/falcon_main.cpp:896-987) over a logits row in HBM.
  * b200_sampling_params is the default chain: llama_sample_repetition_penalty over the last repeat_last_n ids, then temp <= 0 ?
@@ -211,6 +218,13 @@ typedef struct {
  * afterwards, tensor by tensor, under the reference's GGCC tensor names (libfalcon.cpp:1764-1861), e.g.
  * "transformer.h.3.mlp.dense_h_to_4h.weight".  Tensors of layers outside [layer_first, layer_last) are ignored. */
 b200_falcon * b200_falcon_create(const b200_falcon_params * params);
+/* b200_falcon_create with the KV cache stored as kv_ggml_type: GGML_TYPE_F32 (0, what b200_falcon_create does) or GGML_TYPE_F16 (1,
+ * falcon_context_params.f16_kv, libfalcon.h:103).  Any other type: NULL.  An fp16 cache stores K (after RoPE) and V rounded to nearest
+ * even (ggml_fp32_to_fp16 on an F16C host; beyond +-65504 a value becomes +-Inf) and every attention read widens them exactly: the
+ * engine computes what the f32 engine would over a cache whose rows were rounded when they were appended.  It takes half the bytes. */
+b200_falcon * b200_falcon_create_kv(const b200_falcon_params * params, int kv_ggml_type);
+int           b200_falcon_kv_type(const b200_falcon * f);            /* GGML_TYPE_F32 or GGML_TYPE_F16 */
+size_t        b200_falcon_kv_device_bytes(const b200_falcon * f);   /* the cache plus any fp16 copy, all local layers */
 void          b200_falcon_set_tensor(b200_falcon * f, const char * name, int ggml_type, int n_dims,
                                      const int64_t * ne, const void * data);
 /* random-init tensor of the named shape generated on the device (synthetic throughput models) */
@@ -248,11 +262,13 @@ const float * b200_falcon_logits_dev(const b200_falcon * f);
  * logits D2H and the host scan per token (SURVEY 8f-2).  Returns 0 on success. */
 int           b200_falcon_generate_greedy(b200_falcon * f, int32_t first_token, int n_past, int n_steps, int n_ctx_rope, int32_t * tokens_out);
 /* KV cache rows [pos, pos + n) of one (global) layer index, host buffers of n * n_head_kv * head_dim floats each (either may be NULL).
+ * The host rows are f32 for either cache type: an fp16 cache is widened exactly by kv_read and rounded to nearest even by kv_write.
  * The building block of session save / restore (falcon_copy_state_data / falcon_set_state_data, libfalcon.cpp:4313-4490) over the
  * device-resident cache.  Return 0 on success, 1 if the layer is not on this rank or the range leaves [0, n_ctx). */
 int           b200_falcon_kv_read(b200_falcon * f, int layer, int pos, int n, float * k_out, float * v_out);
 int           b200_falcon_kv_write(b200_falcon * f, int layer, int pos, int n, const float * k_in, const float * v_in);
-/* the fp16 copy of the cache that prompt chunks of more than b200_mmv_max_n() tokens attend over (kept only when n_batch exceeds it):
+/* the fp16 copy of the cache that prompt chunks of more than b200_mmv_max_n() tokens attend over (kept only when n_batch exceeds it;
+ * in an fp16 engine k16_out is the K cache itself, always there, and vt16_out only when n_batch exceeds it):
  * positions [pos, pos + n) of one layer as fp16 bit patterns, k16_out [n][n_head_kv][head_dim] and vt16_out [n_head_kv][head_dim][n]
  * (V transposed; either may be NULL).  The range may extend past n_ctx to n_ctx rounded up to 64, the padding of the transposed copy.
  * Return 0 on success, 1 if the engine keeps no such copy, the layer is not on this rank or the range is invalid. */
@@ -262,7 +278,8 @@ int           b200_falcon_kv_shadow_read(b200_falcon * f, int layer, int pos, in
  * load: the number of positions restored (continue evaluating at that n_past), -1 on a missing / truncated / mismatching file. */
 int           b200_falcon_save_kv(b200_falcon * f, const char * path, int n_tokens);
 int           b200_falcon_load_kv(b200_falcon * f, const char * path);
-/* pseudo-random K / V rows for positions [pos, pos + n) of every local layer, generated on the device (long-context throughput runs) */
+/* pseudo-random K / V rows for positions [pos, pos + n) of every local layer, generated on the device (long-context throughput runs;
+ * an fp16 cache holds the same values rounded) */
 int           b200_falcon_kv_fill_random(b200_falcon * f, int pos, int n, uint64_t seed);
 /* b200_falcon_generate_greedy with the sampling chain above run on the device after every step (every rank of a pipeline calls it with
  * the same arguments; the last rank samples).  Returns 0 on success, 1 on bad arguments. */
