@@ -247,8 +247,6 @@ __global__ void kv_shadow_refresh_kernel(const T * __restrict__ kc, const T * __
 
 } // namespace
 
-extern "C" int b200_mmv_max_n(void);
-
 int attention_ctx_pad(int n_ctx) { return (n_ctx + 63) / 64 * 64; }
 size_t attention_shadow_halves(int n_head_kv, int n_ctx) { return (size_t) n_head_kv * 64 * attention_ctx_pad(n_ctx); }     // per layer, for K and for V^T each
 
@@ -267,10 +265,10 @@ void launch_kv_shadow_refresh(const __half * v16, __half * vt16, int n_head_kv, 
     B200_CUDA_CHECK(cudaGetLastError());
 }
 
-// the shapes this kernel takes: an fp16 shadow, head_dim 64, a host n_past, more than b200_mmv_max_n() tokens (B200_ATTN_TC: also fewer)
+// the shapes this kernel takes: an fp16 shadow, head_dim 64, a host n_past, more than MMV_MAX_N tokens (B200_ATTN_TC: also fewer)
 bool attention_ws_covers(const AttnParams & p) {
     if (!p.k16 || !p.vt16 || p.head_dim != D || p.n_past_dev != nullptr || (p.qkv_stride % 4) != 0 || getenv("B200_ATTN_SIMT")) return false;
-    return p.n_tok > b200_mmv_max_n() || getenv("B200_ATTN_TC");     // small batches keep fp32 attention (reassociation-level parity)
+    return p.n_tok > MMV_MAX_N || getenv("B200_ATTN_TC");     // small batches keep fp32 attention (reassociation-level parity)
 }
 void launch_attention_ws(const float * qkv, float * out, int64_t out_stride, const AttnParams & p, cudaStream_t stream) {
     B200_ASSERT(out_stride % 4 == 0);

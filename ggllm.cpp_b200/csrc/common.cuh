@@ -34,6 +34,22 @@ enum : int {
 
 static inline size_t round_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// A device buffer that only grows.  get(need) returns at least `need` bytes; to grow, it waits for `stream` (the buffer's user), frees,
+// and allocates the size rounded up to 1 MB, zeroed.
+struct DevScratch {
+    void * p = nullptr; size_t bytes = 0;
+    void * get(size_t need, cudaStream_t stream) {
+        if (need > bytes) {
+            if (p) { B200_CUDA_CHECK(cudaStreamSynchronize(stream)); B200_CUDA_CHECK(cudaFree(p)); }
+            bytes = round_up(need, 1 << 20);
+            B200_CUDA_CHECK(cudaMalloc(&p, bytes));
+            B200_CUDA_CHECK(cudaMemsetAsync(p, 0, bytes, stream));
+        }
+        return p;
+    }
+    void release() { if (p) B200_CUDA_CHECK(cudaFree(p)); p = nullptr; bytes = 0; }
+};
+
 // One L1/shared-memory split (percent of shared) for every kernel of the decode step.  An SM cannot host kernels that
 // ask for different carve-outs at the same time, so without this the small attention kernels wait for the big
 // mat-vec of the other stream to drain.  25 % of the H100's 228 KB = 57 KB shared, rest L1.

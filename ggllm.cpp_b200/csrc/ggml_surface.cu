@@ -35,19 +35,12 @@ cudaStream_t g_st = nullptr;
 int g_main_device = 0;
 size_t g_scratch_size = 0;       // ggml_cuda_set_scratch_size; 0 => assign_buffers is a no-op (ggml-cuda.cu:3095-3097)
 uint8_t * g_scratch = nullptr; size_t g_scratch_off = 0;
-uint8_t * g_stage = nullptr; size_t g_stage_bytes = 0;      // staging for host-resident operands
+DevScratch g_stage;              // staging for host-resident operands (and the mat-mul's activations)
 std::mutex g_mu;                 // one claimed node at a time (only ith == 0 gets here, but evals may come from several threads)
 
 void ensure_init() { if (!g_initialized) ggml_init_cublas(false); }
 
-uint8_t * stage(size_t bytes) {
-    if (bytes > g_stage_bytes) {
-        if (g_stage) { B200_CUDA_CHECK(cudaStreamSynchronize(g_st)); B200_CUDA_CHECK(cudaFree(g_stage)); }
-        g_stage_bytes = round_up(bytes, 1 << 20);
-        B200_CUDA_CHECK(cudaMalloc(&g_stage, g_stage_bytes));
-    }
-    return g_stage;
-}
+uint8_t * stage(size_t bytes) { return (uint8_t *) g_stage.get(bytes, g_st); }
 
 inline DeviceTensor * owned(const abi::tensor * t) {
     return t->extra ? (DeviceTensor *) ((ggml_tensor_extra_gpu *) t->extra)->data_device[g_main_device] : nullptr;
@@ -81,27 +74,11 @@ void op_mul_mat(const abi::tensor * src0, const abi::tensor * src1, abi::tensor 
     B200_ASSERT(src1->ne[2] == 1 && src1->ne[3] == 1 && src1->ne[0] == w->W.K && dst->ne[0] == w->W.M);
     const int N = (int) src1->ne[1];
     const size_t xb = round_up((size_t) N * w->W.K * 4, 256), yb = round_up((size_t) N * w->W.M * 4, 256);
-    uint8_t * s = stage(xb + yb);
+    uint8_t * s = stage(xb + yb + mul_mat_scratch_bytes(w->W, N));
     const float * x = operand_in(src1, s);
     float * y = result_ptr(dst, s + xb);
-    // the same op the engine uses: activation quantisation + mat-vec (N small) or tensor-core GEMM (N large)
-    const WPlanes & W = w->W;
-    if (W.type == T_F32 || W.type == T_F16) launch_mmv_f(W, x, W.K, N, y, W.M, g_st);
-    else {
-        const int at = act_type_for(W.type);
-        static void * act = nullptr; static size_t act_bytes = 0;
-        const size_t need = actq_bytes(at, W.K, N) + (N > b200_mmv_max_n() ? (size_t) N * W.K * 2 : 0);
-        if (need > act_bytes) { if (act) { B200_CUDA_CHECK(cudaStreamSynchronize(g_st)); B200_CUDA_CHECK(cudaFree(act)); } act_bytes = round_up(need, 1 << 20); B200_CUDA_CHECK(cudaMalloc(&act, act_bytes)); }
-        ActQ A; actq_bind(A, at, W.K, N, act);
-        launch_quantize_act(x, W.K, A, g_st);
-        if (N <= b200_mmv_max_n()) { MmvEpilogue e = { EPI_NONE, nullptr, nullptr }; launch_mmv(W, A, y, W.M, e, g_st); }
-        else {
-            __half * xh = (__half *) ((uint8_t *) act + actq_bytes(at, W.K, N));
-            launch_actq_to_f16(A, xh, W.K, g_st);
-            launch_mmq_gemm(W, xh, W.K, N, y, W.M, 0, g_st);
-        }
-    }
-    dst->meta.cuda_perf_mal_mul_type = N <= b200_mmv_max_n() ? 1 : 16;        // device tag of --debug-timings (ggml.c:18266-18358)
+    launch_mul_mat(w->W, x, w->W.K, N, y, w->W.M, EPI_NONE, s + xb + yb, g_st);             // the op b200_mul_mat runs
+    dst->meta.cuda_perf_mal_mul_type = N <= MMV_MAX_N ? 1 : 16;        // device tag of --debug-timings (ggml.c:18266-18358)
     result_out(dst, y);
 }
 
@@ -271,7 +248,7 @@ bool tk_node(const abi::compute_params * params, abi::tensor * t) {
     if (strcmp(t->name, "result_lm_head") == 0) {
         B200_ASSERT(g_tk.launched && contiguous_f32(t) && nelements(t) == (int64_t) g_tk.N * g_tk.n_vocab);
         falcon_eval_finish(b200_takeover_engine, (float *) t->data);            // falcon_eval_internal reads the logits here (libfalcon.cpp:2538-2549)
-        t->meta.cuda_perf_mal_mul_type = g_tk.N <= b200_mmv_max_n() ? 1 : 16;
+        t->meta.cuda_perf_mal_mul_type = g_tk.N <= MMV_MAX_N ? 1 : 16;
         g_tk.active = false;
     }
     return true;

@@ -5,7 +5,6 @@
 // ---- weights.cu
 size_t wplanes_layout(WPlanes & W, int type, int K, int M);
 void   wplanes_upload(WPlanes & W, int type, int K, int M, const void * host_raw, cudaStream_t stream);
-void   wplanes_from_device_raw(WPlanes & W, int type, int K, int M, const void * dev_raw, cudaStream_t stream);
 void   wplanes_alloc_random(WPlanes & W, int type, int K, int M, uint64_t seed, cudaStream_t stream);
 void   launch_repack_rows(const WPlanes & W, const void * stage_dev, int64_t row0, int64_t nrows, cudaStream_t stream);   // raw blocks of rows [row0, row0 + nrows) -> planes
 void   wplanes_free(WPlanes & W);
@@ -15,7 +14,7 @@ void   launch_dequant_rows(const WPlanes & W, const int32_t * rows_dev, int nrow
 size_t actq_bytes(int act_type, int K, int N);
 void   actq_bind(ActQ & A, int act_type, int K, int N, void * base);          // carve a caller-provided buffer
 void   launch_quantize_act(const float * x, int64_t x_stride, const ActQ & A, cudaStream_t stream);
-void   launch_actq_to_f16(const ActQ & A, __half * dst, int64_t dst_stride, cudaStream_t stream);  // d*q -> fp16 (GEMM operand)
+void   launch_actq_to_f16(const ActQ & A, __half * dst, int64_t dst_stride, cudaStream_t stream);  // d*q -> fp16: b200_actq_to_f16, the reference for A.h
 
 // ---- mmv.cu : y[n][m] = sum_k W[m][k] * xq[n][k], N small (decode), integer dots on quantised activations
 enum { EPI_NONE = 0, EPI_GELU = 1, EPI_ADD2 = 2 };
@@ -41,11 +40,10 @@ bool   mmv_fast_fills_sm(const WPlanes & W);       // its CTAs leave no register
 void   launch_layernorm(const float * x, int64_t x_stride, const float * g, const float * b, float * y, int64_t y_stride,
                         int n, int rows, cudaStream_t stream);              // y = norm(x)*g + b ; g,b may be null (plain ggml_norm)
 // [x = (ra + rb) + x, written back] ; A1 = Q(norm(x)*g1+b1) ; A2 = Q(norm(x)*g2+b2) (optional)
-void   launch_argmax(const float * x, int n, int32_t * out_a, int32_t * out_b, cudaStream_t stream);     // greedy sampling: lowest index on ties
-void   launch_argmax_hist(const float * x, int n, int32_t * out, int32_t * hist, int * step, cudaStream_t stream);  // + hist[(*step)++] = id (graph-replayable)
 void   launch_layernorm_q(float * x, int64_t x_stride, const float * ra, const float * rb, int64_t r_stride,
                           const float * g1, const float * b1, const ActQ * A1,
                           const float * g2, const float * b2, const ActQ * A2, int n, int rows, cudaStream_t stream);
+void   launch_argmax_hist(const float * x, int n, int32_t * out, int32_t * hist, int * step, cudaStream_t stream);  // greedy: lowest index on ties; hist[(*step)++] = id (graph-replayable)
 void   launch_gelu(const float * x, float * y, int64_t n, cudaStream_t stream);
 void   launch_f32_to_f16(const float * x, __half * y, int64_t n, cudaStream_t stream);     // the fp16 activation rows of an F16-weight mat-mul
 void   launch_add(const float * a, const float * b, float * y, int64_t n, cudaStream_t stream);
@@ -55,6 +53,7 @@ void   launch_add_bcast(const float * a, const float * b, float * y, int64_t n, 
 void   launch_scale(const float * a, float s, float * y, int64_t n, cudaStream_t stream);
 struct RopeParams { int n_past; int head_dim; float theta_scale; };
 float  rope_theta_scale_host(int head_dim, int n_ctx_rope, int dynamic_mode, float ntk_alpha, int freq_base);
+float  falcon_rope_theta_scale(int head_dim, int n_ctx_rope, int n_ctx);   // Falcon's settings (libfalcon.cpp:2229-2234); n_ctx_rope 0: n_ctx
 // rotates x[t][h][head_dim] in place (token stride tok_stride, head stride head_dim), position = *n_past_dev + t (or n_past if dev ptr null)
 void   launch_rope_neox(float * x, int n_tok, int n_head, int head_dim, int64_t tok_stride, int n_past, const int * n_past_dev,
                         float theta_scale, cudaStream_t stream);
@@ -132,8 +131,21 @@ size_t attention_shadow_halves(int n_head_kv, int n_ctx);           // halves pe
 void   launch_kv_shadow_refresh(const float * k_cache, const float * v_cache, __half * k16, __half * vt16, int n_head_kv, int n_ctx, int pos, int n, cudaStream_t stream);
 void   launch_kv_shadow_refresh(const __half * v16, __half * vt16, int n_head_kv, int n_ctx, int pos, int n, cudaStream_t stream);   // fp16 cache: V^T only
 
-// ---- gemm.cu : Y[n][m] = sum_k W[m][k] * X[n][k], N large (prompt), wgmma tensor cores
+// ---- gemm.cu : mat-mul dispatch, Y[n][m] = sum_k W[m][k] * X[n][k].  N <= MMV_MAX_N: the mat-vec; above: the prompt GEMM.
+// The launchers return the launches the engine counts: one per mat-vec, quantiser, GELU or GEMM (a GEMM runs in chunks of 512 rows
+// but counts once).
+constexpr int MMV_MAX_N = 8;
+// quantised activations already in A (A.N is set to N); N > MMV_MAX_N needs the fp16 GEMM operand in A.h
+int    launch_mul_mat_q(const WPlanes & W, const ActQ & A, int N, float * y, int64_t y_stride, int epi, cudaStream_t stream);
+// fp32 activation rows: F32 / F16 weights take them as they are (launch_mmv_f, then GELU if asked); quantised weights get them
+// quantised into `scratch` (mul_mat_scratch_bytes(W, N) bytes), fp16 operand included, then launch_mul_mat_q
+int    launch_mul_mat(const WPlanes & W, const float * x, int64_t x_stride, int N, float * y, int64_t y_stride, int epi, void * scratch,
+                      cudaStream_t stream);
+size_t mul_mat_scratch_bytes(const WPlanes & W, int N);
+// the prompt GEMM on fp16 activations: wgmma (gemm_tc.cu) where it covers the shape, the CUDA-core kernel (gemm_simt.cu) elsewhere
 void   launch_mmq_gemm(const WPlanes & W, const __half * X, int64_t x_stride, int N, float * Y, int64_t y_stride, int epi_gelu, cudaStream_t stream);
+void   launch_gemm_simt(const WPlanes & W, const __half * X, int64_t x_stride, int N, float * Y, int64_t y_stride, int epi_gelu, cudaStream_t stream);
+bool   launch_gemm_tc(const WPlanes & W, const __half * X, int64_t x_stride, int N, float * Y, int64_t y_stride, int epi_gelu, cudaStream_t stream);   // false: shape not covered
 
 // ---- sampling.cu: falcon_main's sampling chain on the device (logit bias, repetition / frequency / presence penalties, top-k,
 // tail-free, typical, top-p, temperature, mirostat 1 / 2, MT19937 draw)

@@ -366,6 +366,7 @@ float rope_theta_scale_host(int head_dim, int n_ctx_rope, int dynamic_mode, floa
     } else if (ntk_alpha != 0.0f) alpha = powf(ntk_alpha, head_dim / (head_dim - 2.0));
     return powf(alpha * fb, -2.0f / head_dim);
 }
+float falcon_rope_theta_scale(int head_dim, int n_ctx_rope, int n_ctx) { return rope_theta_scale_host(head_dim, n_ctx_rope ? n_ctx_rope : n_ctx, 1, 2.0f, 0); }
 // pair i of a head at position p, in place
 __device__ __forceinline__ void rope_pair(float * v, int half, int i, int p, float theta_scale) {
     const float theta = rope_theta(p, i, theta_scale);
@@ -469,29 +470,8 @@ void launch_rope_kv_append(float * qkv, float * k_cache, float * v_cache, const 
 }
 
 // ---------------------------------------------------------------------------------------------- greedy sampling
-// arg-max of one logits row; ties -> lowest index (what a sequential `if (x > best)` scan returns); writes the id to two places
-__global__ void __launch_bounds__(1024) argmax_kernel(const float * __restrict__ x, int n, int32_t * __restrict__ out_a, int32_t * __restrict__ out_b) {
-    __shared__ float sv[32]; __shared__ int si[32];
-    float best = -INFINITY; int bi = 0x7fffffff;
-    for (int i = threadIdx.x; i < n; i += blockDim.x) { const float v = x[i]; if (v > best || (v == best && i < bi)) { best = v; bi = i; } }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, best, o); const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
-    }
-    if ((threadIdx.x & 31) == 0) { sv[threadIdx.x >> 5] = best; si[threadIdx.x >> 5] = bi; }
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        best = sv[threadIdx.x]; bi = si[threadIdx.x];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float ov = __shfl_xor_sync(0xffffffffu, best, o); const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
-        }
-        if (threadIdx.x == 0) { if (out_a) *out_a = bi; if (out_b) *out_b = bi; }
-    }
-}
-// graph-replayable form: the id also goes to hist[*step], and the step counter advances
+// arg-max of one logits row; ties -> lowest index (what a sequential `if (x > best)` scan returns).  Graph-replayable: the id also goes
+// to hist[*step], and the step counter advances
 __global__ void __launch_bounds__(1024) argmax_hist_kernel(const float * __restrict__ x, int n, int32_t * __restrict__ out, int32_t * __restrict__ hist, int * __restrict__ step) {
     __shared__ float sv[32]; __shared__ int si[32];
     float best = -INFINITY; int bi = 0x7fffffff;
@@ -515,9 +495,5 @@ __global__ void __launch_bounds__(1024) argmax_hist_kernel(const float * __restr
 }
 void launch_argmax_hist(const float * x, int n, int32_t * out, int32_t * hist, int * step, cudaStream_t stream) {
     argmax_hist_kernel<<<1, 1024, 0, stream>>>(x, n, out, hist, step);
-    B200_CUDA_CHECK(cudaGetLastError());
-}
-void launch_argmax(const float * x, int n, int32_t * out_a, int32_t * out_b, cudaStream_t stream) {
-    argmax_kernel<<<1, 1024, 0, stream>>>(x, n, out_a, out_b);
     B200_CUDA_CHECK(cudaGetLastError());
 }

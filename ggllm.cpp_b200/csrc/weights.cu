@@ -80,18 +80,6 @@ void launch_repack_rows(const WPlanes & W, const void * stage_dev, int64_t row0,
     B200_CUDA_CHECK(cudaGetLastError());
 }
 
-// repack from a raw AoS copy that is already on the device (synthetic models generated on the GPU)
-void wplanes_from_device_raw(WPlanes & W, int type, int K, int M, const void * dev_raw, cudaStream_t stream) {
-    const TypeSpec ts = type_spec(type);
-    wplanes_layout(W, type, K, M);
-    uint8_t * base = nullptr;
-    B200_CUDA_CHECK(cudaMalloc(&base, W.bytes));
-    for (int i = 0; i < ts.n_planes; i++) W.p[i] = base + reinterpret_cast<size_t>(W.p[i]);
-    const int64_t n = (int64_t) M * W.nb;
-    repack_kernel<<<(unsigned) ((n + 255) / 256), 256, 0, stream>>>((const uint8_t *) dev_raw, W, ts, 0, M);
-    B200_CUDA_CHECK(cudaGetLastError());
-}
-
 void wplanes_free(WPlanes & W) {
     if (W.p[0]) B200_CUDA_CHECK(cudaFree(W.p[0]));
     for (int i = 0; i < B200_MAX_PLANES; i++) W.p[i] = nullptr;
