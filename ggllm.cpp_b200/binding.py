@@ -115,11 +115,8 @@ def _np_ptr(a):
     return a.ctypes.data_as(C.c_void_p)
 
 
-def mmv_launch_shape(wtype, K, mode=0):
-    """-> (threads per CTA, pieces per thread, ring depth) of the tuned decode mat-vec, or None for the generic kernel.
-    mode: the activation mode of callers written for the earlier three-mode kernel; only 0 (quantised rows) exists"""
-    if mode != 0:
-        raise ValueError("mmv_launch_shape: only activation mode 0 (quantised rows) exists, got %r" % (mode,))
+def mmv_launch_shape(wtype, K):
+    """-> (threads per CTA, pieces per thread, ring depth) of the tuned decode mat-vec, or None for the generic kernel."""
     s = (C.c_int * 3)()
     return tuple(s) if lib().b200_mmv_launch_shape(wtype, K, s) else None
 

@@ -26,7 +26,6 @@ template <typename E>
 __global__ void __launch_bounds__(ATT_THREADS) attention_kernel(const float * __restrict__ qkv, const E * __restrict__ kc, const E * __restrict__ vc,
                                                                float * __restrict__ out, AttnParams p) {
     extern __shared__ __align__(16) float sm[];
-    trace_begin(p.trace);
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // wo's mat-vec may start prefetching its weights
     const int h = blockIdx.x, D = p.head_dim;
     const int n_past = p.n_past_dev ? *p.n_past_dev : p.n_past;
@@ -82,7 +81,6 @@ __global__ void __launch_bounds__(ATT_THREADS) attention_kernel(const float * __
         for (int g = 1; g < ngrp; g++) r += part[g * D + threadIdx.x];
         out[(size_t) h * D + threadIdx.x] = r;
     }
-    trace_end(p.trace);
 }
 
 // ---- the CUDA-core tier of the split-KV frame (attn_split.cuh), up to attention_long_threshold() keys.  attention_kernel walks a head's
@@ -112,7 +110,6 @@ __device__ __forceinline__ float butterfly16(float (&v)[16], int lane) {
 template <typename E>
 __global__ void __launch_bounds__(SPLIT_THREADS, 6) attn_dec_scores_kernel(const SplitArgs a) {
     __shared__ float wmax[SPLIT_WARPS][SPLIT_G];
-    trace_begin(a.trace);
     const int split = blockIdx.x, kvh = blockIdx.y, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int h0 = kvh * a.G + blockIdx.z * SPLIT_G, G = min(SPLIT_G, a.G - (int) blockIdx.z * SPLIT_G);      // this CTA's query heads: h0 .. h0 + G - 1
     const int n_past = a.n_past_dev ? *a.n_past_dev : a.n_past, T = n_past + 1;
@@ -124,7 +121,7 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 6) attn_dec_scores_kernel(const
 #pragma unroll
     for (int h = 0; h < SPLIT_G; h++)
         q[h] = h < G ? *reinterpret_cast<const float2 *>(a.qkv + (size_t) (h0 + h) * 64 + 2 * lane) : make_float2(0.f, 0.f);
-    if (k_lo >= k_hi) { trace_end(a.trace); return; }            // a split without keys (short context): nothing to score, nobody reads its pmax
+    if (k_lo >= k_hi) return;                                   // a split without keys (short context): nothing to score, nobody reads its pmax
     const float scale = 1.0f / sqrtf(64.0f);
     const size_t kv_row = (size_t) a.n_head_kv * 64;
     // Fused RoPE + KV append (libfalcon.cpp:2229-2281).  A lane holds elements (2l, 2l+1) of a head; NeoX pairs element i < 32 with i + 32,
@@ -183,7 +180,6 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 6) attn_dec_scores_kernel(const
         for (int w = 1; w < SPLIT_WARPS; w++) mx = fmaxf(mx, wmax[w][threadIdx.x]);
         a.pmax[(size_t) (h0 + threadIdx.x) * SPLIT_MAX + split] = mx;
     }
-    trace_end(a.trace);
 }
 
 template <typename E>
@@ -199,7 +195,6 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 6) attn_dec_values_kernel(const
     int k_lo, k_hi; split_range(T, SPLIT_MAX, split, k_lo, k_hi);
     const int nk = k_hi - k_lo;
     const size_t kv_row = (size_t) a.n_head_kv * 64;
-    trace_begin(a.trace);
     const int n_used = splits_used(T, SPLIT_MAX);                 // splits 0 .. n_used - 1 hold keys
     // V rows of EARLIER positions have been in the cache since their own decode steps: the first batch is fetched while the scores kernel
     // still runs (this position's row is appended by that kernel: loaded after the wait)
@@ -273,7 +268,6 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 6) attn_dec_values_kernel(const
     __syncthreads();
     }   // nk > 0
     split_combine(a, oacc, dsum, SPLIT_MAX, n_used, nk, split, h0, G);
-    trace_end(a.trace);
 }
 
 // the values kernel's e array, es[keys per split][SPLIT_G], sized for n_ctx keys
@@ -305,7 +299,7 @@ int attention_long_threshold() {             // read on every call (graph builds
 static int split_tier(const AttnParams & p) {
     if (!split_fits(p)) return 0;
     const bool long_ctx = p.n_past_dev ? p.long_ctx != 0 : p.n_past + 1 > attention_long_threshold();
-    if (long_ctx && !getenv("B200_ATTN_NOLONG")) return 2;
+    if (long_ctx) return 2;
     return !getenv("B200_ATTN_NOSPLIT") && dec_values_smem(p.n_ctx) <= 160 * 1024 ? 1 : 0;
 }
 
@@ -349,9 +343,8 @@ int launch_attention(float * qkv, float * k_cache, float * v_cache, float * out,
             set = true;
         }
         B200_ASSERT(smem <= 200 * 1024);
-        AttnParams pt = p; pt.trace = b200_trace_slot("attention");
-        if (attn_kv16(p)) attention_kernel<<<p.n_head, ATT_THREADS, smem, stream>>>(qkv, (const __half *) p.k16, (const __half *) p.v16, out, pt);
-        else attention_kernel<<<p.n_head, ATT_THREADS, smem, stream>>>(qkv, (const float *) k_cache, (const float *) v_cache, out, pt);
+        if (attn_kv16(p)) attention_kernel<<<p.n_head, ATT_THREADS, smem, stream>>>(qkv, (const __half *) p.k16, (const __half *) p.v16, out, p);
+        else attention_kernel<<<p.n_head, ATT_THREADS, smem, stream>>>(qkv, (const float *) k_cache, (const float *) v_cache, out, p);
         B200_CUDA_CHECK(cudaGetLastError());
         n++;
     } else if (attention_ws_covers(p)) {

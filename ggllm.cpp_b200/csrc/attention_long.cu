@@ -68,7 +68,6 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 4) attn_long_scores_kernel(cons
     __shared__ __align__(16) E ring[SPLIT_WARPS][AL_KR][AL_KB][KS];           // 18 KB (f32) / 9 KB (fp16): K rows in flight
     __shared__ __align__(16) float qs[SPLIT_G][64];                           // this position's query rows, rotated
     __shared__ __align__(16) E knew_s[KS];                                    // this position's key row, rotated (not in the cache yet), as the cache holds it
-    trace_begin(a.trace);
     const int split = blockIdx.x, kvh = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int h0 = kvh * a.G + blockIdx.z * SPLIT_G, G = min(SPLIT_G, a.G - (int) blockIdx.z * SPLIT_G);      // this CTA's query heads: h0 .. h0 + G - 1
     const int n_past = a.n_past_dev ? *a.n_past_dev : a.n_past, T = n_past + 1;
@@ -86,7 +85,7 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 4) attn_long_scores_kernel(cons
     }
     const float * ksrc = a.qkv + (size_t) (a.n_head + kvh) * 64;
     const float ka = ksrc[ri], kb_ = ksrc[ri + 32];
-    if (k_lo >= k_hi) { trace_end(a.trace); return; }            // a split without keys (short context): nothing to score, nobody reads its pmax
+    if (k_lo >= k_hi) return;                                   // a split without keys (short context): nothing to score, nobody reads its pmax
     const int nk = k_hi - k_lo, nst = warp_blocks(nk, warp);
     const int j_new = a.fuse_rope ? n_past - k_lo : -1;           // this position's key is not in the cache yet (another CTA may be writing it right now)
     const size_t kv_row = (size_t) a.n_head_kv * 64;
@@ -189,7 +188,6 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 4) attn_long_scores_kernel(cons
         for (int w = 1; w < SPLIT_WARPS; w++) mx = fmaxf(mx, wmax[w][tid]);
         a.pmax[(size_t) (h0 + tid) * SPLIT_MAX + split] = mx;
     }
-    trace_end(a.trace);
 }
 
 template <typename E>
@@ -208,7 +206,6 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 4) attn_long_values_kernel(cons
     int k_lo, k_hi; split_range(T, a.n_splits, split, k_lo, k_hi);
     const int nk = k_hi - k_lo, nst = warp_blocks(nk, warp);
     const size_t kv_row = (size_t) a.n_head_kv * 64;
-    trace_begin(a.trace);
     const int n_used = splits_used(T, a.n_splits);                // splits 0 .. n_used - 1 hold keys
     const int j_new = n_past - k_lo;                              // this position's V row is appended by the scores kernel: read after the wait
     const int gid = lane >> 2, tig = lane & 3;
@@ -308,7 +305,6 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 4) attn_long_values_kernel(cons
     __syncthreads();
     }   // nk > 0
     split_combine(a, vring, dsum, a.n_splits, n_used, nk, split, h0, G);
-    trace_end(a.trace);
 }
 
 static int g_long_launches = 0;
@@ -316,9 +312,7 @@ extern "C" int b200_attention_long_launches(void) { return g_long_launches; }   
 
 void launch_attention_long(SplitArgs a, cudaStream_t stream) {
     // one wave: as many key splits as SMs divided by the (KV head, head group) pairs -- Falcon-40B 18, 180B 9, 7B 29
-    static int force = -1;
-    if (force < 0) { const char * e = getenv("B200_ATTN_SPLITS"); force = e ? atoi(e) : 0; }
-    a.n_splits = force > 0 ? force : num_sms() / (a.n_head_kv * ((a.G + SPLIT_G - 1) / SPLIT_G));
+    a.n_splits = num_sms() / (a.n_head_kv * ((a.G + SPLIT_G - 1) / SPLIT_G));
     a.n_splits = a.n_splits < 4 ? 4 : a.n_splits > SPLIT_MAX ? SPLIT_MAX : a.n_splits;
     static bool set = false;
     if (!set) {

@@ -27,7 +27,6 @@ struct SplitArgs {
     float * S; float * pmax; double * psum; float * opart; unsigned * ctr;
     int n_head, n_head_kv, G, n_past; const int * n_past_dev; int n_ctx; int64_t qkv_stride;
     int n_splits;
-    unsigned long long * trace;
     ActQ qA; int has_q;          // optional quantised copy of the output row (see AttnParams::qout)
     int fuse_rope; float theta_scale; float * kc_w; float * vc_w; __half * k16; __half * vt16; __half * v16; int ctx_pad;     // see AttnParams::fuse_rope
     int kv16;
@@ -181,14 +180,12 @@ static inline SplitArgs split_args(const float * qkv, const float * k_cache, con
 // scores, then values launched programmatically behind it (it may take the scores kernel's place on the SMs before that grid ends)
 static inline void split_launch(void (*scores)(SplitArgs), void (*values)(SplitArgs), SplitArgs a, size_t values_smem, cudaStream_t stream) {
     const dim3 grid((unsigned) a.n_splits, (unsigned) a.n_head_kv, (unsigned) ((a.G + SPLIT_G - 1) / SPLIT_G));
-    a.trace = b200_trace_slot("attn_scores");
     scores<<<grid, SPLIT_THREADS, 0, stream>>>(a);
     B200_CUDA_CHECK(cudaGetLastError());
-    a.trace = b200_trace_slot("attn_values");
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = grid; cfg.blockDim = dim3(SPLIT_THREADS); cfg.dynamicSmemBytes = values_smem; cfg.stream = stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = getenv("B200_NO_PDL") ? 0 : 1;
+    cfg.attrs = attr; cfg.numAttrs = 1;
     B200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, values, a));
 }

@@ -3,7 +3,6 @@
 #include "../../include/ggml_b200.h"
 #include <mutex>
 #include <cstring>
-#include <vector>
 
 struct b200_weight { WPlanes W; };
 struct b200_actq { ActQ A; void * base; size_t bytes; __half * h; };
@@ -14,36 +13,7 @@ static std::mutex g_mu;
 
 cudaStream_t b200_current_stream() { return g_stream; }
 
-static unsigned long long * g_trace = nullptr; static int g_trace_cap = 0, g_trace_n = 0; static char g_trace_names[4096][24];
-unsigned long long * b200_trace_slot(const char * name) {
-    if (!g_trace || g_trace_n >= g_trace_cap) return nullptr;
-    strncpy(g_trace_names[g_trace_n], name, 23); g_trace_names[g_trace_n][23] = 0;
-    return g_trace + 2 * (g_trace_n++);
-}
-
 extern "C" {
-
-// debugging aid: per-kernel device timeline.  enable(n) allocates n slots and makes every instrumented launch claim one;
-// reset() re-arms the slots (call before replaying a captured graph); dump() copies {start, end} ns pairs and names out.
-void b200_trace_enable(int n_slots) {
-    if (g_trace) { cudaFree(g_trace); g_trace = nullptr; }
-    g_trace_cap = n_slots > 4096 ? 4096 : n_slots; g_trace_n = 0;
-    if (g_trace_cap > 0) B200_CUDA_CHECK(cudaMalloc(&g_trace, (size_t) g_trace_cap * 16));
-}
-void b200_trace_reset(void * stream) {
-    if (!g_trace) return;
-    std::vector<unsigned long long> init((size_t) g_trace_cap * 2);
-    for (int i = 0; i < g_trace_cap; i++) { init[2 * i] = ~0ull; init[2 * i + 1] = 0; }
-    B200_CUDA_CHECK(cudaMemcpy(g_trace, init.data(), init.size() * 8, cudaMemcpyHostToDevice));
-    (void) stream;
-}
-int b200_trace_dump(unsigned long long * out, char * names, int max_slots) {
-    const int n = g_trace_n < max_slots ? g_trace_n : max_slots;
-    B200_CUDA_CHECK(cudaDeviceSynchronize());
-    if (n > 0) B200_CUDA_CHECK(cudaMemcpy(out, g_trace, (size_t) n * 16, cudaMemcpyDeviceToHost));
-    for (int i = 0; i < n; i++) memcpy(names + 24 * i, g_trace_names[i], 24);
-    return n;
-}
 
 int b200_device_count(void) {
     int n = 0;
@@ -189,7 +159,7 @@ static float * attention_scratch(const AttnParams & p) {
 // b200_attention over an f32 cache (kc, vc) or an fp16 one (k16, v16)
 static void attention_op(float * qkv, float * kc, float * vc, __half * k16, __half * v16, float * out, int n_head, int n_head_kv, int head_dim,
                          int n_tok, int n_past, int n_ctx, int n_ctx_rope) {
-    AttnParams p = { n_head, n_head_kv, head_dim, n_tok, n_past, nullptr, n_ctx, (int64_t) (n_head + 2 * n_head_kv) * head_dim, nullptr };
+    AttnParams p = { n_head, n_head_kv, head_dim, n_tok, n_past, nullptr, n_ctx, (int64_t) (n_head + 2 * n_head_kv) * head_dim };
     p.rope_theta_scale = falcon_rope_theta_scale(head_dim, n_ctx_rope, n_ctx);     // libfalcon.cpp:2231-2234
     p.k16 = k16; p.v16 = v16;
     if (n_tok > 1) {
@@ -311,7 +281,7 @@ void b200_layernorm_q(float * x, int64_t x_stride, const float * ra, const float
 // quantize_act (returns 0); the results are the same either way
 static int attention_decode_op(float * qkv, float * kc, float * vc, __half * k16, __half * v16, float * out, int n_head, int n_head_kv, int head_dim,
                                int n_past, int n_ctx, int n_ctx_rope, b200_actq * qout) {
-    AttnParams p = { n_head, n_head_kv, head_dim, 1, n_past, nullptr, n_ctx, (int64_t) (n_head + 2 * n_head_kv) * head_dim, nullptr, nullptr };
+    AttnParams p = { n_head, n_head_kv, head_dim, 1, n_past, nullptr, n_ctx, (int64_t) (n_head + 2 * n_head_kv) * head_dim };
     p.k16 = k16; p.v16 = v16;
     p.fuse_rope = 1; p.rope_theta_scale = falcon_rope_theta_scale(head_dim, n_ctx_rope, n_ctx);      // as the engine: RoPE + append inside
     ActQ Q{}; if (qout) { Q = qout->A; Q.N = 1; p.qout = &Q; }

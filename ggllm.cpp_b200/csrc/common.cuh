@@ -168,11 +168,4 @@ __device__ __forceinline__ void tma_load_1d(void * smem_dst, const void * gmem_s
                  :: "r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 
-// ---- optional device timeline (tools/trace_decode.py): every instrumented kernel gets a slot {min start, max end} in ns
-__device__ __forceinline__ unsigned long long gtimer() { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
-__device__ __forceinline__ void trace_begin(unsigned long long * slot) { if (slot && threadIdx.x == 0) atomicMin(slot, gtimer()); }
-__device__ __forceinline__ void trace_end(unsigned long long * slot) { if (slot && threadIdx.x == 0) atomicMax(slot + 1, gtimer()); }
-
 #endif // __CUDACC__
-
-unsigned long long * b200_trace_slot(const char * name);     // c_api.cu: next slot if tracing is on, else nullptr

@@ -342,7 +342,7 @@ bool launch_gemm_tc(const WPlanes & W, const __half * X, int64_t x_stride, int N
     const int BN = N <= 64 ? 64 : N <= 128 ? 128 : 256;
     // fewer than ~100 tiles cannot fill the 132 SMs of an H100: split K in two (deterministic, see GemmArgs::ksplit)
     const int tiles = (W.M + BM - 1) / BM * ((N + BN - 1) / BN);
-    a.ksplit = (tiles < 100 && !epi_gelu && W.K / BK >= 8 && !getenv("B200_GEMM_NOSPLIT")) ? 2 : 1;
+    a.ksplit = (tiles < 100 && !epi_gelu && W.K / BK >= 8) ? 2 : 1;
     // the two halves add into Y: clear the N rows of M outputs, and only those (columns M .. y_stride-1 belong to the caller)
     if (a.ksplit > 1) B200_CUDA_CHECK(cudaMemset2DAsync(Y, (size_t) y_stride * sizeof(float), 0, (size_t) W.M * sizeof(float), (size_t) N, stream));
     CUtensorMap map;

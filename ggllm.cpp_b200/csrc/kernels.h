@@ -33,7 +33,7 @@ void   launch_mmv_f(const WPlanes & W, const float * x, int64_t x_stride, int N,
 // mmv_fast.cu: the tuned kernel (Q4_K, Q4_0, Q3_K); false = type / K not covered, nothing launched
 bool   launch_mmv_fast(const WPlanes & W, const ActQ & A, float * y, int64_t y_stride, MmvEpilogue e, cudaStream_t stream);
 struct MmvShape { int nt, j, d; };                  // NT threads per CTA, J pieces per thread, ring depth D; nt == 0: generic kernel
-MmvShape mmv_fast_pick_shape(int wtype, int K);     // the shape launch_mmv_fast launches (B200_* switches included)
+MmvShape mmv_fast_pick_shape(int wtype, int K);     // the shape launch_mmv_fast launches
 bool   mmv_fast_supports(int wtype, int K);
 bool   mmv_fast_fills_sm(const WPlanes & W);       // its CTAs leave no registers for a side-stream kernel beside them
 // ---- ops.cu
@@ -66,7 +66,6 @@ struct AttnParams {
     const int * n_past_dev;     // optional device scalar (CUDA-graph replay; one token)
     int n_ctx;                  // KV capacity (row count of the cache)
     int64_t qkv_stride;         // floats between consecutive tokens in the fused QKV buffer
-    unsigned long long * trace; // optional timeline slot (debug)
     const ActQ * qout;          // optional: also emit the output row quantised for the wo mat-mul (its INIT pass)
     // optional fp16 shadow of this layer's cache for the prompt kernel (attention_ws.cu): k16 [n_ctx][n_head_kv][64],
     // vt16 [n_head_kv][64][attention_ctx_pad(n_ctx)] (V transposed); rope_kv_append keeps it in step with the fp32 cache.

@@ -37,7 +37,6 @@ __global__ void __launch_bounds__(NT) __maxnreg__(NT <= 256 ? 96 : 128) mmv_fast
     const int cta = blockIdx.x, nctas = gridDim.x, n = blockIdx.y;
     const int P = W.nb * T::PPB;
 
-    trace_begin(epi.trace);
     if (tid == 0) { mbar_init(bar, 1); mbar_fence_init(); }
     // rows [row0, row1) of this CTA, balanced to +-1
     const int per = W.M / nctas, rem = W.M % nctas;
@@ -105,7 +104,6 @@ __global__ void __launch_bounds__(NT) __maxnreg__(NT <= 256 ? 96 : 128) mmv_fast
             }
         }
     }
-    trace_end(epi.trace);
 }
 
 template <int TYPE, int NT, int J, int D>
@@ -122,7 +120,7 @@ static void launch_cfg(const WPlanes & W, const ActQ & A, float * y, int64_t y_s
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;          // PDL: may start while the previous kernel of the stream drains
     attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = getenv("B200_NO_PDL") ? 0 : 1;
+    cfg.attrs = attr; cfg.numAttrs = 1;
     B200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, mmv_fast_kernel<TYPE, NT, J, D>, W, A, y, y_stride, epi));
 }
 
@@ -134,15 +132,15 @@ static MmvShape pick_shape_t(int K) {
     if (K > 64 * 1024) return {};
     constexpr int D1 = FX<TYPE>::D256;                        // ring depth for one piece per thread; D * J stays constant
     if (P <= 128 && D1 == 4) return { 128, 1, D1 };                                        // 64-weight pieces (Q3_K): K = 8192 is 128 pieces
-    if (P > 128 && P <= 160 && D1 == 8 && !getenv("B200_NO_NT160")) return { 160, 1, D1 }; // Falcon-7B: K = 4544 is 142 pieces
+    if (P > 128 && P <= 160 && D1 == 8) return { 160, 1, D1 };                             // Falcon-7B: K = 4544 is 142 pieces
     if (P <= 256) return { 256, 1, D1 };
     // Falcon-180B (K = 14848: 464 pieces): two 256-thread CTAs at 96 registers instead of one 512-thread CTA at 128 leave a quarter of the
     // register file to the attention kernels of the other stream, as the K = 8192 shape does
-    if (P > 256 && P <= 512 && D1 == 8 && !getenv("B200_NO_NT256J2")) return { 256, 2, D1 / 2 };
+    if (P > 256 && P <= 512 && D1 == 8) return { 256, 2, D1 / 2 };
     if (P <= 512) return { 512, 1, D1 };
     // Falcon-7B's ffn_down (K = 18176: 568 pieces): 3 pieces per thread of a 192-thread CTA use 568 of 576 slots; the 512 x 2 shape
     // below would leave 45 % of its lanes without a piece (and its 128-register CTAs own the whole register file)
-    if (P > 512 && P <= 576 && D1 == 8 && !getenv("B200_NO_NT192")) return { 192, 3, 2 };
+    if (P > 512 && P <= 576 && D1 == 8) return { 192, 3, 2 };
     if (P <= 1024) return { 512, 2, D1 / 2 };
     if (P <= 2048 && D1 == 8) return { 512, 4, 2 };
     return {};
@@ -152,28 +150,36 @@ MmvShape mmv_fast_pick_shape(int wtype, int K) {
     switch (wtype) {
         case T_Q4_K: return pick_shape_t<T_Q4_K>(K);
         case T_Q4_0: return pick_shape_t<T_Q4_0>(K);
-        case T_Q3_K: return !getenv("B200_Q3K_GENERIC") ? pick_shape_t<T_Q3_K>(K) : MmvShape{};
+        case T_Q3_K: return pick_shape_t<T_Q3_K>(K);
     }
     return {};
 }
 
+// exactly the shapes pick_shape_t<TYPE> returns are instantiated
 template <int TYPE>
 static void launch_type(const MmvShape & s, const WPlanes & W, const ActQ & A, float * y, int64_t y_stride, Epi epi, cudaStream_t stream) {
-    constexpr int D1 = FX<TYPE>::D256;
-    if (s.nt == 128) launch_cfg<TYPE, 128, 1, D1>(W, A, y, y_stride, epi, stream);
-    else if (s.nt == 160) launch_cfg<TYPE, 160, 1, D1>(W, A, y, y_stride, epi, stream);
-    else if (s.nt == 256 && s.j == 1) launch_cfg<TYPE, 256, 1, D1>(W, A, y, y_stride, epi, stream);
-    else if (s.nt == 256) launch_cfg<TYPE, 256, 2, D1 / 2>(W, A, y, y_stride, epi, stream);
-    else if (s.nt == 512 && s.j == 1) launch_cfg<TYPE, 512, 1, D1>(W, A, y, y_stride, epi, stream);
-    else if (s.nt == 192) launch_cfg<TYPE, 192, 3, 2>(W, A, y, y_stride, epi, stream);
-    else if (s.nt == 512 && s.j == 2) launch_cfg<TYPE, 512, 2, D1 / 2>(W, A, y, y_stride, epi, stream);
-    else launch_cfg<TYPE, 512, 4, 2>(W, A, y, y_stride, epi, stream);
+    static_assert(FX<TYPE>::D256 == 8 || FX<TYPE>::D256 == 4, "pick_shape_t knows ring depths 8 and 4");
+    if constexpr (FX<TYPE>::D256 == 8) {                                     // Q4_K, Q4_0
+        if (s.nt == 160 && s.j == 1) launch_cfg<TYPE, 160, 1, 8>(W, A, y, y_stride, epi, stream);
+        else if (s.nt == 256 && s.j == 1) launch_cfg<TYPE, 256, 1, 8>(W, A, y, y_stride, epi, stream);
+        else if (s.nt == 256 && s.j == 2) launch_cfg<TYPE, 256, 2, 4>(W, A, y, y_stride, epi, stream);
+        else if (s.nt == 192 && s.j == 3) launch_cfg<TYPE, 192, 3, 2>(W, A, y, y_stride, epi, stream);
+        else if (s.nt == 512 && s.j == 2) launch_cfg<TYPE, 512, 2, 4>(W, A, y, y_stride, epi, stream);
+        else if (s.nt == 512 && s.j == 4) launch_cfg<TYPE, 512, 4, 2>(W, A, y, y_stride, epi, stream);
+        else B200_ASSERT(!"mmv_fast: no kernel for this launch shape");
+    } else {                                                                 // Q3_K
+        if (s.nt == 128 && s.j == 1) launch_cfg<TYPE, 128, 1, 4>(W, A, y, y_stride, epi, stream);
+        else if (s.nt == 256 && s.j == 1) launch_cfg<TYPE, 256, 1, 4>(W, A, y, y_stride, epi, stream);
+        else if (s.nt == 512 && s.j == 1) launch_cfg<TYPE, 512, 1, 4>(W, A, y, y_stride, epi, stream);
+        else if (s.nt == 512 && s.j == 2) launch_cfg<TYPE, 512, 2, 2>(W, A, y, y_stride, epi, stream);
+        else B200_ASSERT(!"mmv_fast: no kernel for this launch shape");
+    }
 }
 
 // returns false if the shape / type is not covered (the caller then uses the generic ring kernel of mmv.cu)
 bool launch_mmv_fast(const WPlanes & W, const ActQ & A, float * y, int64_t y_stride, MmvEpilogue e, cudaStream_t stream) {
-    const char * nm = W.M > 40000 ? "mmv_lmhead" : W.K > 16384 ? "mmv_down" : W.M > 16384 ? "mmv_up" : W.M > 8192 ? "mmv_qkv" : "mmv_wo";
-    Epi epi = { e.kind, e.r1, e.r2, b200_trace_slot(nm), ActQ{}, nullptr, getenv("B200_NO_LATE_WAIT") ? 0 : e.late_wait };
+    Epi epi{};
+    epi.kind = e.kind; epi.r1 = e.r1; epi.r2 = e.r2; epi.late_wait = e.late_wait;
     if (e.qout && e.qctr) {
         B200_ASSERT(A.N == 1 && W.M % 256 == 0 && e.qout->K == W.M && (e.qout->type == T_Q8_K || e.qout->type == T_Q8_0));
         epi.qA = *e.qout; epi.qctr = e.qctr;
@@ -196,7 +202,7 @@ bool mmv_fast_supports(int wtype, int K) {
 // true when the shape chosen for W (3 CTAs of 192 threads at 96 registers) leaves no room on an SM for a side-stream kernel:
 // the decode step then schedules wo BEFORE this mat-vec (engine.cu).  The 512-thread shapes leave ~14k registers: one attention CTA fits.
 bool mmv_fast_fills_sm(const WPlanes & W) {
-    if ((W.type != T_Q4_K && W.type != T_Q4_0) || getenv("B200_NO_NT192")) return false;
+    if (W.type != T_Q4_K && W.type != T_Q4_0) return false;
     const int P = W.K / 32;
     return P > 512 && P <= 576;
 }

@@ -3,7 +3,7 @@
 #include "kernels.h"
 #include "actquant.cuh"
 
-struct Epi { int kind; const float * r1; const float * r2; unsigned long long * trace; ActQ qA; unsigned * qctr; int late_wait; };
+struct Epi { int kind; const float * r1; const float * r2; ActQ qA; unsigned * qctr; int late_wait; };
 
 struct WP { const uint8_t * b0, * b1, * b2, * b3; uint32_t s0, s1, s2, s3; };
 // keeps the compiler from splitting a per-thread plane pointer back into (uniform base) + (thread offset): with an opaque

@@ -102,9 +102,8 @@ template <int ATYPE, int CH>
 __global__ void __launch_bounds__(LNR_THREADS) layernorm_q_reg_kernel(float * __restrict__ x, int64_t x_stride,
         const float * __restrict__ ra, const float * __restrict__ rb, int64_t r_stride,
         const float * __restrict__ g1, const float * __restrict__ b1, ActQ A1,
-        const float * __restrict__ g2, const float * __restrict__ b2, ActQ A2, int has2, int n, unsigned long long * trace) {
+        const float * __restrict__ g2, const float * __restrict__ b2, ActQ A2, int has2, int n) {
     __shared__ double sh[LNR_THREADS / 32];
-    trace_begin(trace);
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // the mat-vecs that follow may start prefetching their weights now
     const int row = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     // launched with programmatic stream serialisation: gamma / beta do not depend on the previous kernel, so they are
@@ -180,7 +179,6 @@ __global__ void __launch_bounds__(LNR_THREADS) layernorm_q_reg_kernel(float * __
             quantize_chunk8<ATYPE>(y, lane, A2, row, e);
         }
     }
-    trace_end(trace);
 }
 
 // Decode (one row): the same LayerNorm + quantisation spread over a thread-block CLUSTER of ceil(n / 1024) <= 8 CTAs x 128 threads,
@@ -202,10 +200,9 @@ __device__ __forceinline__ double ld_dsmem_f64(const double * local, int rank) {
 template <int ATYPE>
 __global__ void __launch_bounds__(LNC_THREADS) layernorm_q_cluster_kernel(float * __restrict__ x, const float * __restrict__ ra, const float * __restrict__ rb,
         const float * __restrict__ g1, const float * __restrict__ b1, ActQ A1,
-        const float * __restrict__ g2, const float * __restrict__ b2, ActQ A2, int has2, int n, unsigned long long * trace) {
+        const float * __restrict__ g2, const float * __restrict__ b2, ActQ A2, int has2, int n) {
     __shared__ double wsum[LNC_THREADS / 32];
     __shared__ double part[2];                                        // this CTA's partial sum / sum of squares, read by the whole cluster
-    trace_begin(trace);
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, C = gridDim.x;
     const int e = ((int) blockIdx.x * LNC_THREADS + threadIdx.x) * 8;
@@ -261,7 +258,6 @@ __global__ void __launch_bounds__(LNC_THREADS) layernorm_q_cluster_kernel(float 
         quantize_chunk8<ATYPE>(y, lane, A2, 0, e, ok);
     }
     cluster_sync_all();                                               // nobody leaves while a peer may still read its `part`
-    trace_end(trace);
 }
 
 void launch_layernorm_q(float * x, int64_t x_stride, const float * ra, const float * rb, int64_t r_stride,
@@ -272,16 +268,15 @@ void launch_layernorm_q(float * x, int64_t x_stride, const float * ra, const flo
     B200_ASSERT(!A2 || A2->type == A1->type);
     const int qblk = A1->type == T_Q8_K ? 256 : 32;                  // whole quantisation blocks per row: idle lanes come in whole blocks
     if (rows == 1 && n % qblk == 0 && (n + LNC_THREADS * 8 - 1) / (LNC_THREADS * 8) <= 8 && !getenv("B200_LN_NOCLUSTER")) {
-        unsigned long long * tr = b200_trace_slot("layernorm_q");
         cudaLaunchConfig_t cfg{};
         cfg.gridDim = dim3((unsigned) ((n + LNC_THREADS * 8 - 1) / (LNC_THREADS * 8))); cfg.blockDim = dim3(LNC_THREADS); cfg.stream = stream;
         cudaLaunchAttribute attr[2];
         attr[0].id = cudaLaunchAttributeClusterDimension; attr[0].val.clusterDim.x = cfg.gridDim.x; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
         attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[1].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr; cfg.numAttrs = getenv("B200_NO_PDL") ? 1 : 2;
+        cfg.attrs = attr; cfg.numAttrs = 2;
         const int has2 = A2 != nullptr;
 #define LNCQ(T) do { static bool set = false; if (!set) { B200_CUDA_CHECK(cudaFuncSetAttribute(layernorm_q_cluster_kernel<T>, cudaFuncAttributePreferredSharedMemoryCarveout, B200_CARVEOUT)); set = true; } \
-        B200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, layernorm_q_cluster_kernel<T>, x, ra, rb, g1, b1, *A1, g2, b2, a2, has2, n, tr)); } while (0)
+        B200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, layernorm_q_cluster_kernel<T>, x, ra, rb, g1, b1, *A1, g2, b2, a2, has2, n)); } while (0)
         switch (A1->type) {
             case T_Q8_0: LNCQ(T_Q8_0); break;
             case T_Q8_1: LNCQ(T_Q8_1); break;
@@ -293,15 +288,14 @@ void launch_layernorm_q(float * x, int64_t x_stride, const float * ra, const flo
     }
     if (n <= 16384 && n % 8 == 0 && !getenv("B200_LN_SMEM")) {
         const bool two = n > 8192;
-        unsigned long long * tr = b200_trace_slot("layernorm_q");
         cudaLaunchConfig_t cfg{};
         cfg.gridDim = dim3((unsigned) rows); cfg.blockDim = dim3(LNR_THREADS); cfg.stream = stream;
         cudaLaunchAttribute attr[1];
         attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr; cfg.numAttrs = getenv("B200_NO_PDL") ? 0 : 1;
+        cfg.attrs = attr; cfg.numAttrs = 1;
         const int has2 = A2 != nullptr;
-#define LNRQ(T) do { if (two) B200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, layernorm_q_reg_kernel<T, 2>, x, x_stride, ra, rb, r_stride, g1, b1, *A1, g2, b2, a2, has2, n, tr)); \
-                     else B200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, layernorm_q_reg_kernel<T, 1>, x, x_stride, ra, rb, r_stride, g1, b1, *A1, g2, b2, a2, has2, n, tr)); } while (0)
+#define LNRQ(T) do { if (two) B200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, layernorm_q_reg_kernel<T, 2>, x, x_stride, ra, rb, r_stride, g1, b1, *A1, g2, b2, a2, has2, n)); \
+                     else B200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, layernorm_q_reg_kernel<T, 1>, x, x_stride, ra, rb, r_stride, g1, b1, *A1, g2, b2, a2, has2, n)); } while (0)
         switch (A1->type) {
             case T_Q8_0: LNRQ(T_Q8_0); break;
             case T_Q8_1: LNRQ(T_Q8_1); break;
@@ -389,7 +383,6 @@ void launch_rope_neox(float * x, int n_tok, int n_head, int head_dim, int64_t to
 
 // fused RoPE(Q) + RoPE(K) + K append + V append (libfalcon.cpp:2229-2281): one CTA per (token, head slot)
 __global__ void rope_kv_append_kernel(float * __restrict__ qkv, float * __restrict__ kc, float * __restrict__ vc, AttnParams p, float theta_scale) {
-    trace_begin(p.trace);
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     const int t = blockIdx.y, slot = blockIdx.x, i = threadIdx.x, D = p.head_dim, half = D / 2;
     const int n_past = p.n_past_dev ? *p.n_past_dev : p.n_past;
@@ -406,7 +399,6 @@ __global__ void rope_kv_append_kernel(float * __restrict__ qkv, float * __restri
             kv_put_v(vc, p.v16, p.vt16, o + i, kvh, i, pos, cp, v[i]); kv_put_v(vc, p.v16, p.vt16, o + i + half, kvh, i + half, pos, cp, v[i + half]);
         }
     }
-    trace_end(p.trace);
 }
 // The same work for a batch of tokens (prompt).  The single-token kernel above recomputes the 32 rotation angles of a position in every
 // one of its (n_head + 2 n_head_kv) x n_tok tiny CTAs and scatters V^T two bytes at a time (at 512 tokens
@@ -464,8 +456,7 @@ void launch_rope_kv_append(float * qkv, float * k_cache, float * v_cache, const 
     dim3 grid((unsigned) (p.n_head + 2 * p.n_head_kv), (unsigned) p.n_tok);
     static bool set = false;
     if (!set) { B200_CUDA_CHECK(cudaFuncSetAttribute(rope_kv_append_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, B200_CARVEOUT)); set = true; }
-    AttnParams pt = p; pt.trace = b200_trace_slot("rope_kv");
-    rope_kv_append_kernel<<<grid, p.head_dim / 2, 0, stream>>>(qkv, k_cache, v_cache, pt, theta_scale);
+    rope_kv_append_kernel<<<grid, p.head_dim / 2, 0, stream>>>(qkv, k_cache, v_cache, p, theta_scale);
     B200_CUDA_CHECK(cudaGetLastError());
 }
 

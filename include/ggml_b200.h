@@ -103,8 +103,7 @@ int    b200_mul_mat_vec_q_chain(const b200_weight * w, const b200_actq * a_in, f
 int    b200_quantize_weights(int ggml_type, const float * x_dev, void * blocks_dev, int64_t n_elems);
 int    b200_mmv_max_n(void);
 /* which kernel the decode mat-vec (b200_mul_mat_vec_q / b200_mul_mat / b200_mul_mat_vec_q_chain) runs for a weight type and
- * row length K, with the B200_NO_NT160 / B200_NO_NT256J2 / B200_NO_NT192 / B200_Q3K_GENERIC switches of the current environment
- * applied.  Returns 1 and nt_j_d = {threads per CTA, pieces per thread, ring depth} for a tuned shape; 0 (nt_j_d = {0, 0, 0})
+ * row length K.  Returns 1 and nt_j_d = {threads per CTA, pieces per thread, ring depth} for a tuned shape; 0 (nt_j_d = {0, 0, 0})
  * when the generic ring kernel runs.  B200_MMV_GENERIC is not applied here. */
 int    b200_mmv_launch_shape(int ggml_type, int64_t K, int * nt_j_d);
 /* the GEMM half alone, on fp16 activations x[n][k] already on the device (what b200_mul_mat does after quantising):

@@ -15,7 +15,6 @@ import mmv_exact as mx
 
 gpu_mark = pytest.mark.gpu
 L4K, L40, L3K = po.Q4_K, po.Q4_0, po.Q3_K
-ENV_SWITCHES = ("B200_NO_NT160", "B200_NO_NT256J2", "B200_NO_NT192")
 RATIOS = collections.defaultdict(float)
 
 # (type, K, M, N, environment switch): one K inside each branch of the launch-shape choice and one on each edge
@@ -26,10 +25,7 @@ FAST = [(L4K, 2048, 301, 1, None), (L4K, 8192, 9216, 1, None), (L4K, 4352, 37, 2
         (L40, 16384, 5, 1, None), (L40, 18176, 4544, 1, None), (L40, 32768, 37, 1, None), (L40, 59392, 37, 2, None),
         (L40, 65536, 37, 1, None), (L40, 65568, 5, 1, None),
         (L3K, 8192, 9216, 1, None), (L3K, 14848, 37, 2, None), (L3K, 32768, 37, 8, None), (L3K, 59392, 37, 1, None),
-        (L3K, 65792, 5, 1, None),
-        (L4K, 14848, 37, 1, "B200_NO_NT256J2"), (L40, 14848, 37, 1, "B200_NO_NT256J2"), (L4K, 4352, 5, 1, "B200_NO_NT160"),
-        (L40, 4544, 37, 1, "B200_NO_NT160"),
-        (L4K, 18432, 37, 1, "B200_NO_NT192"), (L40, 18176, 37, 2, "B200_NO_NT192")]
+        (L3K, 65792, 5, 1, None)]
 # the generic ring kernel (mmv.cu): K with one, two and more work units per row and a ragged last unit, for every type; the
 # types the tuned kernel covers go there through B200_MMV_GENERIC
 GENERIC = [(t, K, 37, 2 if K == 8192 else 1, "B200_MMV_GENERIC" if t in (L4K, L40, L3K) else None)
@@ -39,19 +35,8 @@ GENERIC += [(po.Q6_K, 8192, 9216, 1, None), (po.Q5_K, 32768, 8192, 1, None), (po
 
 
 def _shape(t, K, env):
-    os.environ.pop("B200_MMV_GENERIC", None)
-    old = {k: os.environ.pop(k, None) for k in ENV_SWITCHES}
-    try:
-        if env:
-            os.environ[env] = "1"
-        import ggllm_cpp_b200.binding as b
-        return None if env == "B200_MMV_GENERIC" else b.mmv_launch_shape(t, K)
-    finally:
-        if env:
-            os.environ.pop(env, None)
-        for k, v in old.items():
-            if v is not None:
-                os.environ[k] = v
+    import ggllm_cpp_b200.binding as b
+    return None if env == "B200_MMV_GENERIC" else b.mmv_launch_shape(t, K)
 
 
 def _kernel(shape):
@@ -173,18 +158,17 @@ def test_float_weight_mat_vec_within_exact_bound(gpu, orc, t, K, M):
 
 
 def test_parametrisation_reaches_every_launch_shape():
-    """every (NT, J, D) the launch-shape choice can return for Q4_K, Q4_0 and Q3_K, under any of its switches, is run by
-    test_mat_vec_within_exact_bound; and K past 64 Ki goes to the generic kernel"""
+    """every (NT, J, D) the launch-shape choice can return for Q4_K, Q4_0 and Q3_K is run by test_mat_vec_within_exact_bound;
+    and K past 64 Ki goes to the generic kernel"""
     import ggllm_cpp_b200.binding as b
     if not os.path.exists(b.LIB_PATH):
         b.build()
     possible = set()
     for t in (L4K, L40, L3K):
-        for env in (None,) + ENV_SWITCHES:
-            for K in range(256, 70000, 256):
-                s = _shape(t, K, env)
-                if s is not None:
-                    possible.add((t, s))
+        for K in range(256, 70000, 256):
+            s = _shape(t, K, None)
+            if s is not None:
+                possible.add((t, s))
         assert _shape(t, 65536 + 256, None) is None
     reached = {(c[0], _shape(c[0], c[1], c[4])) for c in FAST}
     missing = possible - reached
