@@ -20,13 +20,13 @@ PART_A = ["b200_event_create", "b200_event_destroy", "b200_event_record", "b200_
           "b200_quantize_act", "b200_actq_download", "b200_actq_alloc_f16", "b200_actq_download_f16", "b200_actq_to_f16", "b200_mul_mat", "b200_mul_mat_f16", "b200_mul_mat_vec_q", "b200_mul_mat_vec_q_chain", "b200_quantize_weights", "b200_mmv_max_n", "b200_mmv_launch_shape", "b200_layernorm",
           "b200_gelu", "b200_add", "b200_rope_neox", "b200_attention", "b200_layernorm_q", "b200_attention_decode", "b200_attention_kv16", "b200_attention_decode_kv16",
           "b200_sampler_create", "b200_sampler_create_chain", "b200_sampler_sample", "b200_sampler_mirostat_mu", "b200_sampler_free",
-          "b200_sampler_tap", "b200_sampler_tap_read"]
+          "b200_sampler_tap", "b200_sampler_tap_read", "b200_token_nll"]
 PART_B = ["b200_falcon_create", "b200_falcon_create_kv", "b200_falcon_kv_type", "b200_falcon_kv_device_bytes", "b200_falcon_set_tensor", "b200_falcon_set_tensor_random", "b200_falcon_load_ggcc",
           "b200_ggcc_read_hparams", "b200_falcon_free", "b200_falcon_weight_bytes", "b200_nccl_unique_id",
           "b200_falcon_init_pipeline", "b200_falcon_eval", "b200_falcon_decode_dev", "b200_falcon_logits_dev", "b200_falcon_generate_greedy",
           "b200_falcon_last_launches", "b200_attention_long_launches", "b200_falcon_last_ms", "b200_falcon_stream", "b200_falcon_profile_matvec",
           "b200_falcon_kv_read", "b200_falcon_kv_write", "b200_falcon_kv_shadow_read", "b200_falcon_kv_fill_random", "b200_falcon_generate", "b200_falcon_generate_chain", "b200_falcon_load_seconds", "b200_falcon_save_kv", "b200_falcon_load_kv",
-          "b200_falcon_tap", "b200_falcon_tap_read"]
+          "b200_falcon_tap", "b200_falcon_tap_read", "b200_falcon_score", "b200_falcon_perplexity"]
 
 
 def build(verbose=False):
@@ -86,6 +86,8 @@ def lib():
             "b200_falcon_logits_dev": (vp, [vp]), "b200_falcon_last_launches": (i32, [vp]), "b200_falcon_last_ms": (f32, [vp]),
             "b200_falcon_stream": (vp, [vp]), "b200_falcon_profile_matvec": (f32, [vp, i32, vp, vp]),
             "b200_falcon_tap": (i32, [vp, i32]), "b200_falcon_tap_read": (i32, [vp, i32, C.c_char_p, vp, sz]),
+            "b200_token_nll": (None, [vp, i32, i32, i64, vp, vp, vp]),
+            "b200_falcon_score": (i32, [vp, vp, i32, i32, i32, vp, vp]), "b200_falcon_perplexity": (i32, [vp, vp, i32, i32, vp, vp]),
         }
         for name, (res, args) in sig.items():
             fn = getattr(L, name)
@@ -158,6 +160,12 @@ class DevBuf:
             self.free()
         except Exception:
             pass
+
+
+def token_nll(logits_dev, n_vocab, n_rows, targets_dev, nll_dev, row_stride=None, stream=None):
+    """b200_token_nll: -log(softmax(row r)[targets[r]]) of device rows logits_dev + r * row_stride into nll_dev[r] (device pointers;
+    target -1 leaves nll_dev[r] as it is, any other target outside [0, n_vocab) writes NaN), enqueued on `stream` (None: the backend's)"""
+    lib().b200_token_nll(logits_dev, n_vocab, n_rows, row_stride or n_vocab, targets_dev, nll_dev, stream)
 
 
 class Weight:
@@ -386,6 +394,31 @@ class Falcon:
         if rc != 0:
             raise RuntimeError("b200_falcon_eval failed (rc=%d)" % rc)
         return out
+
+    def score(self, tokens, n_past, targets, n_ctx_rope=0):
+        """b200_falcon_score: evaluate `tokens` at n_past and return the terms -log p(targets[i]) as float32 [n_tokens], NaN where
+        targets[i] == -1 (not scored); no logits leave the device"""
+        tokens = np.ascontiguousarray(tokens, dtype=np.int32)
+        targets = np.ascontiguousarray(targets, dtype=np.int32)
+        if targets.size != tokens.size:
+            raise ValueError("score: %d targets for %d tokens" % (targets.size, tokens.size))
+        out = np.full(tokens.size, np.nan, np.float32)
+        rc = self.L.b200_falcon_score(self.h, _np_ptr(tokens), tokens.size, n_past, n_ctx_rope, _np_ptr(targets), _np_ptr(out))
+        if rc != 0:
+            raise RuntimeError("b200_falcon_score failed (rc=%d)" % rc)
+        return out
+
+    def perplexity(self, tokens, n_ctx):
+        """b200_falcon_perplexity: falcon_perplexity over `tokens` in chunks of n_ctx -> (ppl after each chunk as float64 [n_chunk],
+        the per-token terms as float32 [n_chunk * (n_ctx - 1 - min(512, n_ctx // 2))])"""
+        tokens = np.ascontiguousarray(tokens, dtype=np.int32)
+        n_chunk = tokens.size // n_ctx if n_ctx > 0 else 0
+        ppl = np.zeros(max(n_chunk, 1), np.float64)
+        nll = np.zeros(max(n_chunk * max(n_ctx - 1 - min(512, n_ctx // 2), 0), 1), np.float32)
+        rc = self.L.b200_falcon_perplexity(self.h, _np_ptr(tokens), tokens.size, n_ctx, _np_ptr(ppl), _np_ptr(nll))
+        if rc < 0:
+            raise RuntimeError("b200_falcon_perplexity: bad n_ctx / tokens, or a pipeline engine")
+        return ppl[:rc], nll[:rc * max(n_ctx - 1 - min(512, n_ctx // 2), 0)]
 
     def generate_greedy(self, first_token, n_past, n_steps, n_ctx_rope=0):
         out = np.zeros(n_steps, dtype=np.int32)

@@ -268,6 +268,10 @@ int b200_sampler_tap_read(const b200_sampler * s, const char * stage, const char
     return sampler_tap_read((const float *) s->tap.p, s->tap_vocab, stage, field, host, bytes) ? 0 : 1;
 }
 
+void b200_token_nll(const float * logits, int n_vocab, int n_rows, int64_t row_stride, const int32_t * targets, float * nll, void * stream) {
+    launch_token_nll(logits, n_vocab, n_rows, row_stride, targets, nll, stream ? (cudaStream_t) stream : g_stream);
+}
+
 // the decode step's LayerNorm node exactly as the engine launches it (cluster kernel for one row of <= 8192 values, register
 // kernel otherwise): [x = (ra + rb) + x] ; a1 = Q(norm(x) * g1 + b1) ; a2 = Q(norm(x) * g2 + b2) (a2 optional)
 void b200_layernorm_q(float * x, int64_t x_stride, const float * ra, const float * rb, const float * g1, const float * b1, b200_actq * a1,

@@ -21,8 +21,10 @@
 #include <sys/mman.h>
 #include <sys/stat.h>
 #include <unistd.h>
+#include <algorithm>
 #include <atomic>
 #include <chrono>
+#include <cmath>
 #include <cstring>
 #include <string>
 #include <thread>
@@ -81,6 +83,7 @@ struct b200_falcon {
     float * attn_dec_scratch = nullptr;            // decode attention: zeroed before the decode graphs are captured
     int32_t * tokens_dev = nullptr; int * n_past_dev = nullptr;
     int32_t * tokens_h = nullptr; int * n_past_h = nullptr; float * logits_h = nullptr; size_t logits_h_floats = 0;
+    int32_t * score_tg = nullptr, * score_tg_h = nullptr; float * score_nll = nullptr, * score_nll_h = nullptr;    // b200_falcon_score's targets / terms [n_batch]
     cudaStream_t s_main = nullptr, s_mlp = nullptr;
     cudaEvent_t e_fork = nullptr, e_join = nullptr, e_t0 = nullptr, e_t1 = nullptr;
     // decode step graphs [tier][which], each with the RoPE theta scale it was captured for.  tier 1: captured with the long-context
@@ -280,6 +283,8 @@ b200_falcon * b200_falcon_create_kv(const b200_falcon_params * p, int kv_ggml_ty
     B200_CUDA_CHECK(cudaMalloc(&f->tok_next, 4)); B200_CUDA_CHECK(cudaMalloc(&f->gen_step, 4));
     B200_CUDA_CHECK(cudaMalloc(&f->gen_hist, (size_t) (p->n_ctx > 0 ? p->n_ctx : 1) * 4));
     B200_CUDA_CHECK(cudaMallocHost(&f->tokens_h, NB * 4)); B200_CUDA_CHECK(cudaMallocHost(&f->n_past_h, 4));
+    B200_CUDA_CHECK(cudaMalloc(&f->score_tg, NB * 4)); B200_CUDA_CHECK(cudaMalloc(&f->score_nll, NB * 4));
+    B200_CUDA_CHECK(cudaMallocHost(&f->score_tg_h, NB * 4)); B200_CUDA_CHECK(cudaMallocHost(&f->score_nll_h, NB * 4));
     f->logits_h_floats = (size_t) f->V; B200_CUDA_CHECK(cudaMallocHost(&f->logits_h, f->logits_h_floats * 4));
     return f;
 }
@@ -520,6 +525,7 @@ void b200_falcon_free(b200_falcon * f) {
     f->attn_scratch.release(); cudaFree(f->actq_mem); cudaFree(f->gen_na); cudaFree(f->gen_nm); cudaFree(f->gen_mm); cudaFree(f->xh_a); cudaFree(f->xh_b); cudaFree(f->xh_m);
     cudaFree(f->tokens_dev); cudaFree(f->n_past_dev); cudaFree(f->q_ctr); cudaFree(f->attn_dec_scratch); cudaFree(f->tap.mem);
     cudaFreeHost(f->tokens_h); cudaFreeHost(f->n_past_h); cudaFreeHost(f->logits_h);
+    cudaFree(f->score_tg); cudaFree(f->score_nll); cudaFreeHost(f->score_tg_h); cudaFreeHost(f->score_nll_h);
     for (auto & tier : f->graph) for (auto & g : tier) if (g.exec) cudaGraphExecDestroy(g.exec);
     cudaFree(f->tok_next); cudaFree(f->gen_hist); cudaFree(f->gen_step); cudaFree(f->sampler_work); sampler_state_free(f->sampler);
     if (f->comm) nccl().CommDestroy(f->comm);
@@ -601,13 +607,15 @@ static void eval_input(b200_falcon * f, int N) {
     } else B200_NCCL_CHECK(nccl().Recv(f->inp, (size_t) N * f->E, ncclFloat, f->hp.rank - 1, f->comm, f->s_main));
 }
 // The end of an eval: the residual adds of the last local layer (:2399-2400), then on the last rank the head over rows
-// [logits_rows_from, N) and, in the generation-step graph, the sampled id; on every other rank the rows go on to the next one.
+// [logits_rows_from, N) (none when logits_rows_from == N: a scoring batch without a scored row) and, in the generation-step graph,
+// the sampled id; on every other rank the rows go on to the next one.
 // fold_add: a quantised head's LayerNorm kernel does the adds (one kernel less on the decode step)
 static void eval_output(b200_falcon * f, int N, int logits_rows_from, bool fold_add) {
     const bool fold = fold_add && f->last && !f->generic_head && f->NL > 0;
     if (f->NL > 0 && !fold) { launch_add3(f->dn, f->ao, f->inp, f->inp, (int64_t) N * f->E, f->s_main); f->launches++; }
     if (!f->last) { B200_NCCL_CHECK(nccl().Send(f->inp, (size_t) N * f->E, ncclFloat, f->hp.rank + 1, f->comm, f->s_main)); return; }
-    enqueue_head(f, f->inp + (size_t) logits_rows_from * f->E, N - logits_rows_from, fold ? f->dn : nullptr, fold ? f->ao : nullptr, f->s_main);
+    if (logits_rows_from < N)
+        enqueue_head(f, f->inp + (size_t) logits_rows_from * f->E, N - logits_rows_from, fold ? f->dn : nullptr, fold ? f->ao : nullptr, f->s_main);
     tap_head(f, N, N - logits_rows_from);
     ring_token_out(f);
 }
@@ -789,17 +797,42 @@ static cudaGraphExec_t decode_graph(b200_falcon * f, int which, int tier, float 
     return f->graph[tier][which].exec;
 }
 
+// b200_falcon_eval's argument checks: 0, 1 (batch or positions outside the engine's n_batch / n_ctx), 2 (a token id outside the vocabulary)
+static int eval_args(const b200_falcon * f, const int32_t * tokens, int n_tokens, int n_past) {
+    if (n_tokens <= 0 || n_past < 0 || n_past + n_tokens > f->hp.n_ctx || n_tokens > (f->hp.n_batch > 0 ? f->hp.n_batch : 1)) return 1;
+    if (f->first) {                                  // token ids index the embedding matrix: reject anything outside it (ggml_get_rows asserts, ggml.c:11990)
+        if (!tokens) return 1;
+        for (int i = 0; i < n_tokens; i++) if (tokens[i] < 0 || tokens[i] >= f->V) return 2;
+    }
+    return 0;
+}
+
+// One batch of b200_falcon_score / b200_falcon_perplexity on s_main, tokens already in tokens_dev: the eval of N tokens at n_past, then
+// the scoring kernel over the rows whose device target is not -1, terms into nll_dev.  scored: some target is not -1; the head then runs
+// over all N rows, the rows b200_falcon_eval(all_logits = 1) runs it over (the mat-vec head up to MMV_MAX_N rows, the GEMM above: a
+// suffix of the rows could take the other path and round differently), otherwise not at all.  One token replays the decode step graph
+// as b200_falcon_eval does, minus its logits copy.
+static void enqueue_score_batch(b200_falcon * f, int N, int n_past, float theta, const int32_t * targets_dev, float * nll_dev, bool scored) {
+    if (N == 1) {
+        set_i32_kernel<<<1, 1, 0, f->s_main>>>(f->n_past_dev, n_past);
+        const cudaGraphExec_t g = decode_graph(f, G_DEVICE, tier_of(n_past), theta);
+        B200_CUDA_CHECK(cudaGraphLaunch(g, f->s_main));
+        f->launches = f->graph_launches;
+    } else {
+        f->launches = 0;
+        enqueue_eval(f, N, n_past, theta, false, scored ? 0 : N);
+    }
+    if (scored) { launch_token_nll(f->logits, f->V, N, f->V, targets_dev, nll_dev, f->s_main); f->launches++; }
+}
+
 extern "C" {
 
 // The eval in two halves: enqueue everything (returns at once: the GPU works while the caller does something else) / wait and hand the
 // logits over.  b200_falcon_eval is begin + finish; the operator hook (ggml_surface.cu) calls begin at the graph's first ROPE node and
 // finish at "result_lm_head", so the reference's walk over its remaining ~2000 graph nodes overlaps the device work.
 extern "C++" int falcon_eval_begin(b200_falcon * f, const int32_t * tokens, int n_tokens, int n_past, int n_ctx_rope, int all_logits) {
-    if (n_tokens <= 0 || n_past < 0 || n_past + n_tokens > f->hp.n_ctx || n_tokens > (f->hp.n_batch > 0 ? f->hp.n_batch : 1)) return 1;
-    if (f->first) {                                  // token ids index the embedding matrix: reject anything outside it (ggml_get_rows asserts, ggml.c:11990)
-        if (!tokens) return 1;
-        for (int i = 0; i < n_tokens; i++) if (tokens[i] < 0 || tokens[i] >= f->V) return 2;
-    }
+    const int rc = eval_args(f, tokens, n_tokens, n_past);
+    if (rc != 0) return rc;
     const float theta = falcon_rope_theta_scale(f->D, n_ctx_rope, f->hp.n_ctx);         // libfalcon.cpp:2229-2234
     if (n_tokens == 1) {
         f->tokens_h[0] = tokens ? tokens[0] : 0; *f->n_past_h = n_past;
@@ -840,6 +873,80 @@ int b200_falcon_eval(b200_falcon * f, const int32_t * tokens, int n_tokens, int 
     if (rc != 0) return rc;
     falcon_eval_finish(f, logits);
     return 0;
+}
+
+int b200_falcon_score(b200_falcon * f, const int32_t * tokens, int n_tokens, int n_past, int n_ctx_rope, const int32_t * targets, float * nll) {
+    if (f->hp.world > 1) return 1;
+    const int rc = eval_args(f, tokens, n_tokens, n_past);
+    if (rc != 0) return rc;
+    if (!targets) return 3;
+    bool scored = false;
+    for (int i = 0; i < n_tokens; i++) {
+        if (targets[i] < -1 || targets[i] >= f->V) return 3;
+        scored = scored || targets[i] >= 0;
+    }
+    if (scored && !nll) return 1;
+    const float theta = falcon_rope_theta_scale(f->D, n_ctx_rope, f->hp.n_ctx);
+    const size_t bytes = (size_t) n_tokens * 4;
+    memcpy(f->tokens_h, tokens, bytes); memcpy(f->score_tg_h, targets, bytes);
+    B200_CUDA_CHECK(cudaMemcpyAsync(f->tokens_dev, f->tokens_h, bytes, cudaMemcpyHostToDevice, f->s_main));
+    B200_CUDA_CHECK(cudaMemcpyAsync(f->score_tg, f->score_tg_h, bytes, cudaMemcpyHostToDevice, f->s_main));
+    B200_CUDA_CHECK(cudaEventRecord(f->e_t0, f->s_main));
+    enqueue_score_batch(f, n_tokens, n_past, theta, f->score_tg, f->score_nll, scored);
+    B200_CUDA_CHECK(cudaEventRecord(f->e_t1, f->s_main));
+    if (scored) B200_CUDA_CHECK(cudaMemcpyAsync(f->score_nll_h, f->score_nll, bytes, cudaMemcpyDeviceToHost, f->s_main));
+    B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
+    for (int i = 0; i < n_tokens; i++) if (targets[i] >= 0) nll[i] = f->score_nll_h[i];
+    B200_CUDA_CHECK(cudaEventElapsedTime(&f->last_ms, f->e_t0, f->e_t1));
+    return 0;
+}
+
+// falcon_perplexity's loop (falcon_perplexity.cpp:28-123) over b200_falcon_score's batches.  The token ids and the per-row targets
+// (-1 outside the scored range) go H2D once; every batch copies its ids D2D into the eval's input; the terms stay on the device until
+// the end, and the host sums them in double in the reference's order.
+int b200_falcon_perplexity(b200_falcon * f, const int32_t * tokens, int n_tokens, int n_ctx, double * ppl, float * nll) {
+    if (f->hp.world > 1 || n_ctx < 2 || n_ctx > f->hp.n_ctx || n_tokens < 0 || (n_tokens > 0 && !tokens)) return -1;
+    for (int i = 0; i < n_tokens; i++) if (tokens[i] < 0 || tokens[i] >= f->V) return -1;
+    const int n_chunk = n_tokens / n_ctx;
+    if (n_chunk == 0) return 0;
+    const int n_batch = f->hp.n_batch > 0 ? f->hp.n_batch : 1, first = std::min(512, n_ctx / 2);
+    const size_t n_used = (size_t) n_chunk * n_ctx;
+    std::vector<int32_t> tg(n_used, -1);
+    for (size_t c = 0; c < (size_t) n_chunk; c++)
+        for (int k = first; k < n_ctx - 1; k++) tg[c * n_ctx + k] = tokens[c * n_ctx + k + 1];
+    int32_t * tok_d = nullptr, * tg_d = nullptr; float * terms_d = nullptr;
+    B200_CUDA_CHECK(cudaMalloc(&tok_d, n_used * 4)); B200_CUDA_CHECK(cudaMalloc(&tg_d, n_used * 4)); B200_CUDA_CHECK(cudaMalloc(&terms_d, n_used * 4));
+    B200_CUDA_CHECK(cudaMemcpyAsync(tok_d, tokens, n_used * 4, cudaMemcpyHostToDevice, f->s_main));
+    B200_CUDA_CHECK(cudaMemcpyAsync(tg_d, tg.data(), n_used * 4, cudaMemcpyHostToDevice, f->s_main));
+    const float theta = falcon_rope_theta_scale(f->D, n_ctx, f->hp.n_ctx);          // the reference's context is made with n_ctx
+    int launches = 0;
+    B200_CUDA_CHECK(cudaEventRecord(f->e_t0, f->s_main));
+    for (size_t c = 0; c < (size_t) n_chunk; c++)
+        for (int p0 = 0; p0 < n_ctx; p0 += n_batch) {
+            const int N = std::min(n_ctx - p0, n_batch);
+            const size_t off = c * n_ctx + p0;
+            B200_CUDA_CHECK(cudaMemcpyAsync(f->tokens_dev, tok_d + off, (size_t) N * 4, cudaMemcpyDeviceToDevice, f->s_main));
+            enqueue_score_batch(f, N, p0, theta, tg_d + off, terms_d + off, std::max(p0, first) < std::min(p0 + N, n_ctx - 1));
+            launches += f->launches;
+        }
+    B200_CUDA_CHECK(cudaEventRecord(f->e_t1, f->s_main));
+    std::vector<float> terms(n_used);
+    B200_CUDA_CHECK(cudaMemcpyAsync(terms.data(), terms_d, n_used * 4, cudaMemcpyDeviceToHost, f->s_main));
+    B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
+    B200_CUDA_CHECK(cudaEventElapsedTime(&f->last_ms, f->e_t0, f->e_t1));
+    f->launches = launches;
+    cudaFree(tok_d); cudaFree(tg_d); cudaFree(terms_d);
+    double sum = 0.0; size_t count = 0;
+    for (size_t c = 0; c < (size_t) n_chunk; c++) {
+        for (int k = first; k < n_ctx - 1; k++) {
+            const float t = terms[c * n_ctx + k];
+            sum += t;                                                       // nll += -std::log(prob)
+            if (nll) nll[count] = t;
+            count++;
+        }
+        if (ppl) ppl[c] = std::exp(sum / (double) count);
+    }
+    return n_chunk;
 }
 
 int b200_falcon_decode_dev(b200_falcon * f, const int32_t * token_dev, int n_past, int n_ctx_rope) {

@@ -168,6 +168,9 @@ void   launch_sample(const float * logits, int n_vocab, const SamplerParams & p,
                      float * tap, cudaStream_t stream);
 size_t sampler_tap_bytes(int n_vocab);
 bool   sampler_tap_read(const float * tap, int n_vocab, const char * stage, const char * field, void * host, size_t bytes);
+// falcon_perplexity's per-token term -log(softmax(row)[target]) of rows [0, n_rows) (row r at logits + r * row_stride): target -1
+// skips the row (nll[r] unwritten), a target outside [0, n_vocab) writes NaN (b200_token_nll)
+void   launch_token_nll(const float * logits, int n_vocab, int n_rows, int64_t row_stride, const int32_t * targets, float * nll, cudaStream_t stream);
 
 // ---- engine.cu (internal, C++ linkage): adopt a matrix that is already resident in the planar layout (no copy, not freed by the engine)
 struct b200_falcon;

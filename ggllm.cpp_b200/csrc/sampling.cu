@@ -463,7 +463,66 @@ __global__ void __launch_bounds__(NT) sample_kernel(const float * __restrict__ l
     }
 }
 
+// ---- falcon_perplexity's score of one row (examples/falcon_perplexity/falcon_perplexity.cpp:12-26, 113-115): with m = max_i l[i],
+//   e[i] = expf(l[i] - m),  S = (((0.0 + e[0]) + e[1]) + ...) + e[V-1] in double, one rounding per add,  p = (float) (e[t] / S),
+//   nll = -logf(p)                                                                          (p == 0 gives +Inf)
+// The double sum is the reference's sequential loop, so it is one dependent chain of V adds per row.  One CTA per row: warps 1..7
+// produce e[] a chunk ahead into a double buffer in shared memory while lane 0 of warp 0 adds the previous chunk in id order, so the
+// chain runs back to back.  The producers also widen e[] to double, so the summing thread issues nothing but loads and adds (a
+// conversion to or from fp64 is a quarter-rate instruction, which would cost more than the add itself).  The max is order-free;
+// e[t] is recomputed from the same float operands.
+constexpr int NLL_NT = 256, NLL_CHUNK = 2048;
+
+__global__ void __launch_bounds__(NLL_NT) token_nll_kernel(const float * __restrict__ logits, int n_vocab, int64_t row_stride,
+                                                           const int32_t * __restrict__ targets, float * __restrict__ nll) {
+    __shared__ __align__(16) double buf[2][NLL_CHUNK];
+    __shared__ float s_max[NLL_NT / 32];
+    const int row = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int t = targets[row];
+    if (t == -1) return;                                               // not scored: the slot stays as it is
+    if (t < 0 || t >= n_vocab) { if (tid == 0) nll[row] = NAN; return; }
+    const float * l = logits + (size_t) row * row_stride;
+    float m = -INFINITY;
+    for (int i = tid; i < n_vocab; i += NLL_NT) { const float v = l[i]; m = v > m ? v : m; }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { const float v = __shfl_xor_sync(0xffffffffu, m, o); m = v > m ? v : m; }
+    if (lane == 0) s_max[warp] = m;
+    __syncthreads();
+    m = s_max[0];
+#pragma unroll
+    for (int w = 1; w < NLL_NT / 32; w++) m = s_max[w] > m ? s_max[w] : m;
+    double S = 0.0;
+    const int n_chunks = (n_vocab + NLL_CHUNK - 1) / NLL_CHUNK;
+    for (int c = 0; c <= n_chunks; c++) {                              // step c: produce chunk c, add up chunk c - 1
+        if (warp > 0) {
+            const int c0 = c * NLL_CHUNK, n = min(NLL_CHUNK, n_vocab - c0);
+            for (int i = tid - 32; i < n; i += NLL_NT - 32) buf[c & 1][i] = (double) ref_expf(__fsub_rn(l[c0 + i], m));
+        } else if (tid == 0 && c > 0) {
+            const int n = min(NLL_CHUNK, n_vocab - (c - 1) * NLL_CHUNK);
+            const double * b = buf[(c - 1) & 1];
+            const double2 * b2 = (const double2 *) b;
+            int i = 0;
+#pragma unroll 8
+            for (; i + 2 <= n; i += 2) { const double2 v = b2[i >> 1]; S = __dadd_rn(S, v.x); S = __dadd_rn(S, v.y); }
+            if (i < n) S = __dadd_rn(S, b[i]);
+        }
+        __syncthreads();
+    }
+    if (tid == 0) {
+        const float et = ref_expf(__fsub_rn(l[t], m));
+        const float p = __double2float_rn(__ddiv_rn((double) et, S));  // probs[i] /= sum_exp: float / double, stored as float
+        nll[row] = -ref_logf(p);
+    }
+}
+
 } // namespace
+
+void launch_token_nll(const float * logits, int n_vocab, int n_rows, int64_t row_stride, const int32_t * targets, float * nll, cudaStream_t stream) {
+    B200_ASSERT(n_vocab > 0 && n_rows >= 0 && row_stride >= n_vocab);
+    if (n_rows == 0) return;
+    token_nll_kernel<<<n_rows, NLL_NT, 0, stream>>>(logits, n_vocab, row_stride, targets, nll);
+    B200_CUDA_CHECK(cudaGetLastError());
+}
 
 SamplerState * sampler_state_alloc() { SamplerState * s = nullptr; B200_CUDA_CHECK(cudaMalloc(&s, sizeof(SamplerState))); return s; }
 void sampler_state_free(SamplerState * s) { if (s) B200_CUDA_CHECK(cudaFree(s)); }

@@ -198,6 +198,15 @@ void           b200_sampler_free(b200_sampler * s);
 int            b200_sampler_tap(b200_sampler * s, int on);
 int            b200_sampler_tap_read(const b200_sampler * s, const char * stage, const char * field, void * host, size_t bytes);
 
+/* ---- scoring on the device: falcon_perplexity's per-token term (examples/falcon_perplexity/falcon_perplexity.cpp:12-26, 113-115).
+ * For row r (logits_dev + r * row_stride, n_vocab floats) with target t = targets_dev[r]:
+ *   m = max_i l[i];  e[i] = expf(l[i] - m) (float);  S = (((0.0 + e[0]) + e[1]) + ...) + e[n_vocab - 1] (double, sequential, in id order);
+ *   p = (float) ((double) e[t] / S);  nll_dev[r] = -logf(p) (float; p == 0 gives +Inf).
+ * expf / logf are correctly rounded (the sampler's), where glibc's differ from that in the last bit at times.  t == -1 skips the row
+ * (nll_dev[r] unwritten); any other t outside [0, n_vocab) writes NaN.  Enqueued on `cuda_stream` (NULL = the backend stream). */
+void           b200_token_nll(const float * logits_dev, int n_vocab, int n_rows, int64_t row_stride, const int32_t * targets_dev,
+                              float * nll_dev, void * cuda_stream);
+
 /* ========================================= part B: Falcon eval path ====================================== */
 
 typedef struct b200_falcon b200_falcon;
@@ -251,6 +260,22 @@ void          b200_falcon_init_pipeline(b200_falcon * f, const void * id128);
  * In a pipeline every rank calls it; only the last rank's `logits` are written.  Returns 0 on success. */
 int           b200_falcon_eval(b200_falcon * f, const int32_t * tokens, int n_tokens, int n_past, int n_ctx_rope,
                                float * logits, int all_logits);
+/* b200_falcon_eval that scores its rows on the device instead of returning logits (single GPU): targets[i] in [0, n_vocab) scores
+ * row i -- nll[i] (host) receives b200_token_nll's term for it -- and -1 skips it (nll[i] untouched).  No logits cross PCIe.
+ * A batch with a scored row runs the final LayerNorm and lm_head over all n_tokens rows, exactly as b200_falcon_eval(all_logits = 1)
+ * does, so the scored logits are bit for bit that call's; a batch without one runs no head.  One token replays the decode step graph.
+ * Returns b200_falcon_eval's codes (0, 1, 2), 3 for a target outside [-1, n_vocab) (checked before anything runs), 1 on a pipeline
+ * engine (world > 1) or a NULL nll with a scored row. */
+int           b200_falcon_score(b200_falcon * f, const int32_t * tokens, int n_tokens, int n_past, int n_ctx_rope,
+                                const int32_t * targets, float * nll);
+/* falcon_perplexity (examples/falcon_perplexity/falcon_perplexity.cpp:28-123) over tokens[0, n_tokens): n_chunk = n_tokens / n_ctx
+ * chunks (the tail is dropped); chunk c evaluates tokens[c n_ctx, (c + 1) n_ctx) in batches of the engine's n_batch at n_past
+ * 0, n_batch, ... with the rope context n_ctx and no BOS substitution, and scores rows k in [min(512, n_ctx / 2), n_ctx - 1) against
+ * tokens[c n_ctx + k + 1] through b200_falcon_score.  The terms are summed in double in k order over all chunks so far and
+ * ppl[c] = exp(sum / count) after chunk c (what the reference prints as [c+1]).  nll (optional) receives the terms, n_chunk *
+ * (n_ctx - 1 - min(512, n_ctx / 2)) floats; ppl (optional) n_chunk doubles.  The tokens go H2D once and only the terms come back.
+ * Returns n_chunk (>= 0), or -1 for n_ctx < 2, n_ctx above the engine's n_ctx, a token outside the vocabulary or world > 1. */
+int           b200_falcon_perplexity(b200_falcon * f, const int32_t * tokens, int n_tokens, int n_ctx, double * ppl, float * nll);
 /* device-resident decode step for throughput measurement: token id already on the device, logits stay on the
  * device (b200_falcon_logits_dev).  Same kernels/graph as b200_falcon_eval minus the two PCIe copies. */
 int           b200_falcon_decode_dev(b200_falcon * f, const int32_t * token_dev, int n_past, int n_ctx_rope);   /* 0 = ok, 1 = n_past outside [0, n_ctx) */
