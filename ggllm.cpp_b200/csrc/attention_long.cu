@@ -90,7 +90,7 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 4) attn_long_scores_kernel(cons
     const int j_new = a.fuse_rope ? n_past - k_lo : -1;           // this position's key is not in the cache yet (another CTA may be writing it right now)
     const size_t kv_row = (size_t) a.n_head_kv * 64;
     const int gid = lane >> 2, tig = lane & 3;
-    const E * kp = split_cache<E>(a.kc) + (size_t) kvh * 64 + 16 * tig + (size_t) k_lo * kv_row;
+    const E * kp = kv_k<E>(a.kv) + (size_t) kvh * 64 + 16 * tig + (size_t) k_lo * kv_row;
     auto issue = [&](int i) {                                     // lane copies dims 16 tig .. 16 tig + 15 of key gid of the block
         if (i < nst) {
             const int jj = (i * SPLIT_WARPS + warp) * AL_KB + gid;
@@ -129,8 +129,8 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 4) attn_long_scores_kernel(cons
                 const size_t o = ((size_t) n_past * a.n_head_kv + kvh) * 64;
                 const float * vsrc = a.qkv + (size_t) (a.n_head + a.n_head_kv + kvh) * 64;
                 const float v0 = vsrc[ri], v1 = vsrc[ri + 32];
-                kv_put_k(a.kc_w, a.k16, o + ri, y0); kv_put_k(a.kc_w, a.k16, o + ri + 32, y1);
-                kv_put_v(a.vc_w, a.v16, a.vt16, o + ri, kvh, ri, n_past, a.ctx_pad, v0); kv_put_v(a.vc_w, a.v16, a.vt16, o + ri + 32, kvh, ri + 32, n_past, a.ctx_pad, v1);
+                kv_put_k(a.kv, o + ri, y0); kv_put_k(a.kv, o + ri + 32, y1);
+                kv_put_v(a.kv, o + ri, kvh, ri, n_past, v0); kv_put_v(a.kv, o + ri + 32, kvh, ri + 32, n_past, v1);
             }
         }
     }
@@ -209,7 +209,7 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 4) attn_long_values_kernel(cons
     const int n_used = splits_used(T, a.n_splits);                // splits 0 .. n_used - 1 hold keys
     const int j_new = n_past - k_lo;                              // this position's V row is appended by the scores kernel: read after the wait
     const int gid = lane >> 2, tig = lane & 3;
-    const E * vp = split_cache<E>(a.vc) + (size_t) kvh * 64 + 16 * tig + (size_t) k_lo * kv_row;
+    const E * vp = kv_v<E>(a.kv) + (size_t) kvh * 64 + 16 * tig + (size_t) k_lo * kv_row;
     const float * S0 = a.S + (size_t) (h0 + min(gid, G - 1)) * a.n_ctx + k_lo, * S1 = a.S + (size_t) (h0 + min(gid + 8, G - 1)) * a.n_ctx + k_lo;
     E (*vr)[AL_KB][VS] = reinterpret_cast<E (*)[AL_KB][VS]>(vring[warp]);
     auto issue = [&](int i, bool v, bool s) {
@@ -246,7 +246,7 @@ __global__ void __launch_bounds__(SPLIT_THREADS, 4) attn_long_values_kernel(cons
     for (int i = 0; i < AL_KR - 1; i++) issue(i, false, true);    // their scores, together with the split maxima: one round trip
     const bool has_new = j_new >= 0 && j_new < nk;
     E2 vnew{};
-    if (has_new) vnew = *reinterpret_cast<const E2 *>(split_cache<E>(a.vc) + (size_t) kvh * 64 + 2 * lane + (size_t) (k_lo + j_new) * kv_row);
+    if (has_new) vnew = *reinterpret_cast<const E2 *>(kv_v<E>(a.kv) + (size_t) kvh * 64 + 2 * lane + (size_t) (k_lo + j_new) * kv_row);
     if (tid < SPLIT_G) {
         float mx = -INFINITY;
         if (tid < G) for (int s = 0; s < n_used; s++) mx = fmaxf(mx, a.pmax[(size_t) (h0 + tid) * SPLIT_MAX + s]);
@@ -322,6 +322,6 @@ void launch_attention_long(SplitArgs a, cudaStream_t stream) {
         set = true;
     }
     g_long_launches++;
-    if (a.kv16) split_launch(attn_long_scores_kernel<__half>, attn_long_values_kernel<__half>, a, 0, stream);
+    if (kv_f16(a.kv)) split_launch(attn_long_scores_kernel<__half>, attn_long_values_kernel<__half>, a, 0, stream);
     else split_launch(attn_long_scores_kernel<float>, attn_long_values_kernel<float>, a, 0, stream);
 }

@@ -1,5 +1,5 @@
 // attention_prefill.cu -- causal grouped-query attention for a batch of N > 1 new tokens (prompt processing) where attention_ws.cu
-// does not apply (N <= 8, no fp16 shadow, head_dim != 64), over an f32 or an fp16 cache (template on the element type E).
+// does not apply (N <= 8, no fp16 shadow, head_dim != 64), over the layer's KvCache, f32 or fp16 (template on the element type E).
 //
 // Same arithmetic contract as attention.cu (libfalcon.cpp:2285-2366, ggml.c:12389-12458): fp32 scores, softmax with the
 // row's GLOBAL maximum subtracted before an fp16-LUT exp, the sum accumulated in double, probabilities scaled by
@@ -17,7 +17,7 @@
 #define PTHREADS 256
 
 struct PrefillArgs {
-    const float * qkv; const void * kc; const void * vc; float * out; float * S; float * inv;     // cache: f32, or fp16 (the kernels' E)
+    const float * qkv; KvCache kv; float * out; float * S; float * inv;     // kv: read as the kernels' E
     int n_head, n_head_kv, G, D, n_tok, n_past, T;      // T = n_past + n_tok
     int64_t qkv_stride, out_stride, s_stride;           // s_stride = T rounded up to 64
     int rows;                                           // G * n_tok rows per kv head
@@ -26,8 +26,9 @@ struct PrefillArgs {
 // row -> (token, head)
 __device__ __forceinline__ void row_to(const PrefillArgs & a, int g, int row, int & t, int & h) { t = row / a.G; h = g * a.G + row % a.G; }
 
+// 4 CTAs per SM (64 registers): left to itself, ptxas takes 74-78 registers for this kernel, depending on the size of its parameters
 template <typename E>
-__global__ void __launch_bounds__(PTHREADS) prefill_scores_kernel(const PrefillArgs a) {
+__global__ void __launch_bounds__(PTHREADS, 4) prefill_scores_kernel(const PrefillArgs a) {
     __shared__ float sq[PT][PT + 1];      // [row][d]
     __shared__ float sk[PT][PT + 1];      // [key][d]
     __shared__ float smax[PT];
@@ -50,7 +51,7 @@ __global__ void __launch_bounds__(PTHREADS) prefill_scores_kernel(const PrefillA
         __syncthreads();
         for (int i = threadIdx.x; i < PT * PT; i += PTHREADS) {
             const int kk = i / PT, d = i % PT, key = k0 + kk;
-            sk[kk][d] = (key < a.T && d < a.D) ? kv_ld(static_cast<const E *>(a.kc) + ((size_t) key * a.n_head_kv + g) * a.D + d) : 0.f;
+            sk[kk][d] = (key < a.T && d < a.D) ? kv_ld(kv_k<E>(a.kv) + ((size_t) key * a.n_head_kv + g) * a.D + d) : 0.f;
         }
         __syncthreads();
         float acc[4][4] = {};
@@ -118,7 +119,7 @@ __global__ void __launch_bounds__(PTHREADS) prefill_pv_kernel(const PrefillArgs 
             }
             sp[r][kk] = p;
             const int kv = i / PT, d = i % PT, key2 = k0 + kv;
-            sv[kv][d] = (key2 < a.T && d < a.D) ? kv_ld(static_cast<const E *>(a.vc) + ((size_t) key2 * a.n_head_kv + g) * a.D + d) : 0.f;
+            sv[kv][d] = (key2 < a.T && d < a.D) ? kv_ld(kv_v<E>(a.kv) + ((size_t) key2 * a.n_head_kv + g) * a.D + d) : 0.f;
         }
         __syncthreads();
 #pragma unroll 8
@@ -147,13 +148,11 @@ size_t attention_prefill_scratch_bytes(int n_head, int n_tok, int T) {
     return (size_t) n_head * n_tok * s_stride * 4 + (size_t) n_head * n_tok * 4 + 256;
 }
 
-void launch_attention_prefill(const float * qkv, const float * k_cache, const float * v_cache, float * out, int64_t out_stride,
-                              const AttnParams & p, float * scratch, cudaStream_t stream) {
+void launch_attention_prefill(const float * qkv, float * out, int64_t out_stride, const AttnParams & p, float * scratch, cudaStream_t stream) {
     B200_ASSERT(p.head_dim <= PT && p.n_past_dev == nullptr);
     PrefillArgs a;
-    const bool kv16 = attn_kv16(p);
-    a.qkv = qkv; a.out = out;
-    a.kc = kv16 ? (const void *) p.k16 : k_cache; a.vc = kv16 ? (const void *) p.v16 : v_cache;
+    const bool kv16 = kv_f16(p.kv);
+    a.qkv = qkv; a.kv = p.kv; a.out = out;
     a.n_head = p.n_head; a.n_head_kv = p.n_head_kv; a.G = p.n_head / p.n_head_kv; a.D = p.head_dim; a.n_tok = p.n_tok; a.n_past = p.n_past;
     a.T = p.n_past + p.n_tok; a.qkv_stride = p.qkv_stride; a.out_stride = out_stride; a.s_stride = (a.T + 63) / 64 * 64;
     a.rows = a.G * p.n_tok;

@@ -232,16 +232,15 @@ PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
 }
 
 // cache rows [pos, pos + n) -> the fp16 planes the prompt kernel reads (used when a cache was filled by something other than
-// rope_kv_append: session restore, kv_write, the per-operator C ABI).  fp32 cache: k16 and vt16; fp16 cache (T = __half): vt16 only
-template <typename T>
-__global__ void kv_shadow_refresh_kernel(const T * __restrict__ kc, const T * __restrict__ vc, __half * __restrict__ k16, __half * __restrict__ vt16,
-                                         int n_head_kv, int ctx_pad, int pos, int n) {
+// rope_kv_append: session restore, kv_write, the per-operator C ABI).  f32 cache (E = float): k16 and vt16; fp16 cache: vt16 only
+template <typename E>
+__global__ void kv_shadow_refresh_kernel(const KvCache c, int n_head_kv, int pos, int n) {
     const int64_t total = (int64_t) n * n_head_kv * 64;
     for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t) gridDim.x * blockDim.x) {
         const int d = (int) (i % 64), h = (int) ((i / 64) % n_head_kv), p = pos + (int) (i / (64 * n_head_kv));
         const size_t src = ((size_t) p * n_head_kv + h) * 64 + d;
-        if (kc) k16[src] = __float2half_rn(kv_ld(kc + src));
-        vt16[((size_t) h * 64 + d) * ctx_pad + p] = __float2half_rn(kv_ld(vc + src));
+        if (sizeof(E) == 4) c.k16[src] = __float2half_rn(c.k[src]);
+        c.vt16[((size_t) h * 64 + d) * c.ctx_pad + p] = __float2half_rn(kv_ld(kv_v<E>(c) + src));
     }
 }
 
@@ -250,24 +249,18 @@ __global__ void kv_shadow_refresh_kernel(const T * __restrict__ kc, const T * __
 int attention_ctx_pad(int n_ctx) { return (n_ctx + 63) / 64 * 64; }
 size_t attention_shadow_halves(int n_head_kv, int n_ctx) { return (size_t) n_head_kv * 64 * attention_ctx_pad(n_ctx); }     // per layer, for K and for V^T each
 
-void launch_kv_shadow_refresh(const float * k_cache, const float * v_cache, __half * k16, __half * vt16, int n_head_kv, int n_ctx, int pos, int n, cudaStream_t stream) {
-    if (n <= 0) return;
+void launch_kv_shadow_refresh(const KvCache & c, int n_head_kv, int pos, int n, cudaStream_t stream) {
+    if (n <= 0 || !c.vt16) return;           // no shadow (an f32 cache's k16 exists exactly when vt16 does)
     const int64_t total = (int64_t) n * n_head_kv * 64;
     const unsigned grid = (unsigned) (total / 256 + 1 > 132 * 8 ? 132 * 8 : total / 256 + 1);
-    kv_shadow_refresh_kernel<<<grid, 256, 0, stream>>>(k_cache, v_cache, k16, vt16, n_head_kv, attention_ctx_pad(n_ctx), pos, n);
-    B200_CUDA_CHECK(cudaGetLastError());
-}
-void launch_kv_shadow_refresh(const __half * v16, __half * vt16, int n_head_kv, int n_ctx, int pos, int n, cudaStream_t stream) {
-    if (n <= 0) return;
-    const int64_t total = (int64_t) n * n_head_kv * 64;
-    const unsigned grid = (unsigned) (total / 256 + 1 > 132 * 8 ? 132 * 8 : total / 256 + 1);
-    kv_shadow_refresh_kernel<__half><<<grid, 256, 0, stream>>>(nullptr, v16, nullptr, vt16, n_head_kv, attention_ctx_pad(n_ctx), pos, n);
+    if (kv_f16(c)) kv_shadow_refresh_kernel<__half><<<grid, 256, 0, stream>>>(c, n_head_kv, pos, n);
+    else kv_shadow_refresh_kernel<float><<<grid, 256, 0, stream>>>(c, n_head_kv, pos, n);
     B200_CUDA_CHECK(cudaGetLastError());
 }
 
 // the shapes this kernel takes: an fp16 shadow, head_dim 64, a host n_past, more than MMV_MAX_N tokens (B200_ATTN_TC: also fewer)
 bool attention_ws_covers(const AttnParams & p) {
-    if (!p.k16 || !p.vt16 || p.head_dim != D || p.n_past_dev != nullptr || (p.qkv_stride % 4) != 0 || getenv("B200_ATTN_SIMT")) return false;
+    if (!p.kv.k16 || !p.kv.vt16 || p.head_dim != D || p.n_past_dev != nullptr || (p.qkv_stride % 4) != 0 || getenv("B200_ATTN_SIMT")) return false;
     return p.n_tok > MMV_MAX_N || getenv("B200_ATTN_TC");     // small batches keep fp32 attention (reassociation-level parity)
 }
 void launch_attention_ws(const float * qkv, float * out, int64_t out_stride, const AttnParams & p, cudaStream_t stream) {
@@ -276,7 +269,7 @@ void launch_attention_ws(const float * qkv, float * out, int64_t out_stride, con
     a.qkv = qkv; a.out = out;
     a.n_head_kv = p.n_head_kv; a.G = p.n_head / p.n_head_kv; a.n_tok = p.n_tok; a.n_past = p.n_past; a.T = p.n_past + p.n_tok;
     a.rows = a.G * p.n_tok; a.qkv_stride = p.qkv_stride; a.out_stride = out_stride;
-    const int ctx_pad = attention_ctx_pad(p.n_ctx);
+    const int ctx_pad = p.kv.ctx_pad;
     // Both maps end at key T, not at n_ctx / ctx_pad: TMA zero-fills the rest of the last key tile.  Cache rows >= T are stale (an earlier
     // sequence, kv_write, load_kv) and may hold NaN or, for an fp32 value beyond 65504, Inf in the shadow; the masked probabilities are
     // exact zeros, but 0 x NaN and 0 x Inf in the P V product are NaN.
@@ -285,7 +278,7 @@ void launch_attention_ws(const float * qkv, float * out, int64_t out_stride, con
         const cuuint64_t gdim[3] = { 64, (cuuint64_t) p.n_head_kv, (cuuint64_t) a.T };
         const cuuint64_t gstr[2] = { 128, (cuuint64_t) p.n_head_kv * 128 };
         const cuuint32_t box[3] = { 64, 1, 128 }, estr[3] = { 1, 1, 1 };
-        const CUresult rc = get_encode()(&kmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void *) p.k16, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+        const CUresult rc = get_encode()(&kmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void *) p.kv.k16, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (rc != CUDA_SUCCESS) { fprintf(stderr, "b200: cuTensorMapEncodeTiled(k16) failed (%d)\n", (int) rc); exit(1); }
     }
@@ -293,7 +286,7 @@ void launch_attention_ws(const float * qkv, float * out, int64_t out_stride, con
         const cuuint64_t gdim[3] = { (cuuint64_t) a.T, 64, (cuuint64_t) p.n_head_kv };
         const cuuint64_t gstr[2] = { (cuuint64_t) ctx_pad * 2, (cuuint64_t) ctx_pad * 128 };
         const cuuint32_t box[3] = { 64, 64, 1 }, estr[3] = { 1, 1, 1 };
-        const CUresult rc = get_encode()(&vmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void *) p.vt16, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+        const CUresult rc = get_encode()(&vmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void *) p.kv.vt16, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (rc != CUDA_SUCCESS) { fprintf(stderr, "b200: cuTensorMapEncodeTiled(vt16) failed (%d)\n", (int) rc); exit(1); }
     }

@@ -23,19 +23,18 @@
 #define SPLIT_MIN_KEYS 64
 
 struct SplitArgs {
-    const float * qkv; const void * kc; const void * vc; float * out;     // the cache: f32, or __half with kv16 (the kernels' element type)
+    const float * qkv; float * out;
+    KvCache kv;                  // the layer's cache (kernels.h); its element type is the kernels' E
     float * S; float * pmax; double * psum; float * opart; unsigned * ctr;
     int n_head, n_head_kv, G, n_past; const int * n_past_dev; int n_ctx; int64_t qkv_stride;
     int n_splits;
     ActQ qA; int has_q;          // optional quantised copy of the output row (see AttnParams::qout)
-    int fuse_rope; float theta_scale; float * kc_w; float * vc_w; __half * k16; __half * vt16; __half * v16; int ctx_pad;     // see AttnParams::fuse_rope
-    int kv16;
+    int fuse_rope; float theta_scale;     // see AttnParams::fuse_rope
 };
-template <typename T> __device__ __forceinline__ const T * split_cache(const void * p) { return reinterpret_cast<const T *>(p); }
 // the fused append of this position's rows (elements e, e + 1 of K and V head kvh): every plane there is, through kernels.h's writer
 __device__ __forceinline__ void split_append2(const SplitArgs & a, size_t o, int kvh, int e, int n_past, float2 k, float2 v) {
-    kv_put_k(a.kc_w, a.k16, o, k.x); kv_put_k(a.kc_w, a.k16, o + 1, k.y);
-    kv_put_v(a.vc_w, a.v16, a.vt16, o, kvh, e, n_past, a.ctx_pad, v.x); kv_put_v(a.vc_w, a.v16, a.vt16, o + 1, kvh, e + 1, n_past, a.ctx_pad, v.y);
+    kv_put_k(a.kv, o, k.x); kv_put_k(a.kv, o + 1, k.y);
+    kv_put_v(a.kv, o, kvh, e, n_past, v.x); kv_put_v(a.kv, o + 1, kvh, e + 1, n_past, v.y);
 }
 
 __device__ __forceinline__ int split_keys(int T, int ns) { return max(SPLIT_MIN_KEYS, (T + ns - 1) / ns); }
@@ -165,16 +164,13 @@ static inline size_t split_layout(const AttnParams & p, float * scratch, SplitAr
     return o_opart + align256((size_t) SPLIT_MAX * p.n_head * 64 * 4);
 }
 // the kernels' arguments for p; n_splits and the quantised output are the caller's
-static inline SplitArgs split_args(const float * qkv, const float * k_cache, const float * v_cache, float * out, const AttnParams & p, float * scratch) {
+static inline SplitArgs split_args(const float * qkv, float * out, const AttnParams & p, float * scratch) {
     SplitArgs a{};
     split_layout(p, scratch, &a);
-    a.kv16 = attn_kv16(p);
-    a.qkv = qkv; a.out = out;
-    if (a.kv16) { a.kc = p.k16; a.vc = p.v16; } else { a.kc = k_cache; a.vc = v_cache; }
+    a.qkv = qkv; a.out = out; a.kv = p.kv;
     a.n_head = p.n_head; a.n_head_kv = p.n_head_kv; a.G = p.n_head / p.n_head_kv; a.n_past = p.n_past; a.n_past_dev = p.n_past_dev; a.n_ctx = p.n_ctx;
     a.qkv_stride = p.qkv_stride;
-    a.fuse_rope = p.fuse_rope; a.theta_scale = p.rope_theta_scale; a.kc_w = const_cast<float *>(k_cache); a.vc_w = const_cast<float *>(v_cache);
-    a.k16 = p.k16; a.vt16 = p.vt16; a.v16 = p.v16; a.ctx_pad = attention_ctx_pad(p.n_ctx);
+    a.fuse_rope = p.fuse_rope; a.theta_scale = p.rope_theta_scale;
     return a;
 }
 // scores, then values launched programmatically behind it (it may take the scores kernel's place on the SMs before that grid ends)

@@ -156,12 +156,12 @@ static float * attention_scratch(const AttnParams & p) {
     B200_CUDA_CHECK(cudaMemsetAsync(sc, 0, ATTN_CTR_BYTES, g_stream));
     return sc;
 }
-// b200_attention over an f32 cache (kc, vc) or an fp16 one (k16, v16)
-static void attention_op(float * qkv, float * kc, float * vc, __half * k16, __half * v16, float * out, int n_head, int n_head_kv, int head_dim,
-                         int n_tok, int n_past, int n_ctx, int n_ctx_rope) {
+// b200_attention over the caller's cache: f32 (k, v) or fp16 (k16, v16)
+static void attention_op(float * qkv, const KvCache & kv, float * out, int n_head, int n_head_kv, int head_dim, int n_tok, int n_past, int n_ctx,
+                         int n_ctx_rope) {
     AttnParams p = { n_head, n_head_kv, head_dim, n_tok, n_past, nullptr, n_ctx, (int64_t) (n_head + 2 * n_head_kv) * head_dim };
     p.rope_theta_scale = falcon_rope_theta_scale(head_dim, n_ctx_rope, n_ctx);     // libfalcon.cpp:2231-2234
-    p.k16 = k16; p.v16 = v16;
+    p.kv = kv; p.kv.ctx_pad = attention_ctx_pad(n_ctx);
     if (n_tok > 1) {
         // the warp-specialised wgmma kernel reads fp16 K and V^T planes: built here from the caller's cache (the engine keeps them up to
         // date token by token instead; an fp16 cache is its own K plane); the RoPE + append kernel writes the new rows
@@ -170,19 +170,19 @@ static void attention_op(float * qkv, float * kc, float * vc, __half * k16, __ha
         if (need) {
             __half * sh = (__half *) shadow.get(2 * need * sizeof(__half), g_stream);
             B200_CUDA_CHECK(cudaMemsetAsync(sh, 0, 2 * need * sizeof(__half), g_stream));
-            p.vt16 = sh + need;
-            if (v16) launch_kv_shadow_refresh(v16, p.vt16, n_head_kv, n_ctx, 0, n_past, g_stream);
-            else { p.k16 = sh; launch_kv_shadow_refresh(kc, vc, p.k16, p.vt16, n_head_kv, n_ctx, 0, n_past, g_stream); }
+            p.kv.vt16 = sh + need;
+            if (!kv_f16(p.kv)) p.kv.k16 = sh;
+            launch_kv_shadow_refresh(p.kv, n_head_kv, 0, n_past, g_stream);
         }
     }
-    launch_attention(qkv, kc, vc, out, (int64_t) n_head * head_dim, p, attention_scratch(p), g_stream);
+    launch_attention(qkv, out, (int64_t) n_head * head_dim, p, attention_scratch(p), g_stream);
 }
 void b200_attention(float * qkv, float * kc, float * vc, float * out, int n_head, int n_head_kv, int head_dim, int n_tok, int n_past, int n_ctx, int n_ctx_rope) {
-    attention_op(qkv, kc, vc, nullptr, nullptr, out, n_head, n_head_kv, head_dim, n_tok, n_past, n_ctx, n_ctx_rope);
+    attention_op(qkv, { kc, vc }, out, n_head, n_head_kv, head_dim, n_tok, n_past, n_ctx, n_ctx_rope);
 }
 void b200_attention_kv16(float * qkv, uint16_t * k16, uint16_t * v16, float * out, int n_head, int n_head_kv, int head_dim, int n_tok, int n_past,
                          int n_ctx, int n_ctx_rope) {
-    attention_op(qkv, nullptr, nullptr, (__half *) k16, (__half *) v16, out, n_head, n_head_kv, head_dim, n_tok, n_past, n_ctx, n_ctx_rope);
+    attention_op(qkv, { nullptr, nullptr, (__half *) k16, (__half *) v16 }, out, n_head, n_head_kv, head_dim, n_tok, n_past, n_ctx, n_ctx_rope);
 }
 
 // ---- stand-alone sampler over a logits row on the device (the engine's generation loop runs the same kernel inside its step graph)
@@ -283,23 +283,23 @@ void b200_layernorm_q(float * x, int64_t x_stride, const float * ra, const float
 // the decode step's attention node as the engine launches it: RoPE + KV append, split-KV scores / values kernels, and the output row
 // also quantised for the wo mat-mul -- by the attention combine step when the Q8 blocks fit the head groups (returns 1), else by
 // quantize_act (returns 0); the results are the same either way
-static int attention_decode_op(float * qkv, float * kc, float * vc, __half * k16, __half * v16, float * out, int n_head, int n_head_kv, int head_dim,
-                               int n_past, int n_ctx, int n_ctx_rope, b200_actq * qout) {
+static int attention_decode_op(float * qkv, const KvCache & kv, float * out, int n_head, int n_head_kv, int head_dim, int n_past, int n_ctx,
+                               int n_ctx_rope, b200_actq * qout) {
     AttnParams p = { n_head, n_head_kv, head_dim, 1, n_past, nullptr, n_ctx, (int64_t) (n_head + 2 * n_head_kv) * head_dim };
-    p.k16 = k16; p.v16 = v16;
+    p.kv = kv; p.kv.ctx_pad = attention_ctx_pad(n_ctx);
     p.fuse_rope = 1; p.rope_theta_scale = falcon_rope_theta_scale(head_dim, n_ctx_rope, n_ctx);      // as the engine: RoPE + append inside
     ActQ Q{}; if (qout) { Q = qout->A; Q.N = 1; p.qout = &Q; }
     bool folded = false;
-    launch_attention(qkv, kc, vc, out, (int64_t) n_head * head_dim, p, attention_scratch(p), g_stream, &folded);
+    launch_attention(qkv, out, (int64_t) n_head * head_dim, p, attention_scratch(p), g_stream, &folded);
     return folded ? 1 : 0;
 }
 int b200_attention_decode(float * qkv, float * kc, float * vc, float * out, int n_head, int n_head_kv, int head_dim, int n_past, int n_ctx,
                           int n_ctx_rope, b200_actq * qout) {
-    return attention_decode_op(qkv, kc, vc, nullptr, nullptr, out, n_head, n_head_kv, head_dim, n_past, n_ctx, n_ctx_rope, qout);
+    return attention_decode_op(qkv, { kc, vc }, out, n_head, n_head_kv, head_dim, n_past, n_ctx, n_ctx_rope, qout);
 }
 int b200_attention_decode_kv16(float * qkv, uint16_t * k16, uint16_t * v16, float * out, int n_head, int n_head_kv, int head_dim, int n_past,
                                int n_ctx, int n_ctx_rope, b200_actq * qout) {
-    return attention_decode_op(qkv, nullptr, nullptr, (__half *) k16, (__half *) v16, out, n_head, n_head_kv, head_dim, n_past, n_ctx, n_ctx_rope, qout);
+    return attention_decode_op(qkv, { nullptr, nullptr, (__half *) k16, (__half *) v16 }, out, n_head, n_head_kv, head_dim, n_past, n_ctx, n_ctx_rope, qout);
 }
 
 } // extern "C"

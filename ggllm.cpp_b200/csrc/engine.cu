@@ -71,10 +71,9 @@ struct b200_falcon {
     std::vector<Layer> layers;
     WPlanes tok_emb{}, lm_head{};
     float * lnf_g = nullptr, * lnf_b = nullptr;
-    int kv_type = T_F32;                        // the cache's element type: T_F32, or T_F16 (b200_falcon_create_kv)
-    float * k_cache = nullptr, * v_cache = nullptr;                        // f32 cache (null in an fp16 engine)
-    __half * k16 = nullptr, * vt16 = nullptr; size_t shadow_layer = 0;      // fp16 K plane for the prompt kernel (attention_ws.cu) -- the K cache itself in an fp16 engine -- and V^T (only when n_batch > 8); shadow_layer: halves per layer of each plane
-    __half * v16 = nullptr;                                                // fp16 engine: the V cache
+    // the KV cache (f32, or fp16 from b200_falcon_create_kv), every layer in one allocation per plane: layer 0's view (kv_layer).  The
+    // prompt kernel's V^T, and an f32 cache's fp16 K shadow, exist only when n_batch > 8.  shadow_layer: halves per layer of each fp16 plane
+    KvCache kv{}; size_t shadow_layer = 0;
     // activation arena
     float * inp = nullptr, * qkv = nullptr, * att = nullptr, * ao = nullptr, * up = nullptr, * dn = nullptr, * logits = nullptr;
     void * actq_mem = nullptr; ActQ xa{}, xm{}, xatt{}, xup{}, xf{};
@@ -115,19 +114,29 @@ struct b200_falcon {
                  std::vector<int> rotated; } tap;                // rotated[l]: RoPE ran in place on qkv (not inside the attention kernels)
 };
 
-// Local layer l's slice of the KV cache.  f32 engine: k / v [n_ctx][n_head_kv][head_dim] f32, rows of kv_row() floats, and k16 / vt16 its
-// fp16 shadow in the layout of AttnParams::k16 / vt16 (null when the engine keeps none).  fp16 engine: k16 / v16 [n_ctx][n_head_kv][head_dim]
-// are the cache (k / v null), vt16 as above.
-struct KvLayer { float * k, * v; __half * k16, * vt16, * v16; };
+// Local layer l's slice of the KV cache (kernels.h's KvCache): f32 rows of kv_row() floats, fp16 planes shadow_layer halves apart.
 static size_t kv_row(const b200_falcon * f) { return (size_t) f->HKV * f->D; }
-static KvLayer kv_layer(const b200_falcon * f, int l) {
-    KvLayer c = { nullptr, nullptr, nullptr, nullptr, nullptr };
+static KvCache kv_layer(const b200_falcon * f, int l) {
+    KvCache c = f->kv;
     const size_t off = (size_t) l * f->hp.n_ctx * kv_row(f), off16 = (size_t) l * f->shadow_layer;
-    if (f->k_cache) { c.k = f->k_cache + off; c.v = f->v_cache + off; }
-    if (f->k16) c.k16 = f->k16 + off16;
-    if (f->vt16) c.vt16 = f->vt16 + off16;
-    if (f->v16) c.v16 = f->v16 + off16;
+    if (c.k) { c.k += off; c.v += off; }
+    if (c.k16) c.k16 += off16;
+    if (c.v16) c.v16 += off16;
+    if (c.vt16) c.vt16 += off16;
     return c;
+}
+// f32 host rows <-> a cache plane (kv_read / kv_write)
+static void kv_d2h(float * dst, const float * src, size_t n) { B200_CUDA_CHECK(cudaMemcpy(dst, src, n * 4, cudaMemcpyDeviceToHost)); }
+static void kv_d2h(float * dst, const __half * src, size_t n) {
+    std::vector<__half> h(n);
+    B200_CUDA_CHECK(cudaMemcpy(h.data(), src, n * 2, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < n; i++) dst[i] = __half2float(h[i]);
+}
+static void kv_h2d(float * dst, const float * src, size_t n) { B200_CUDA_CHECK(cudaMemcpy(dst, src, n * 4, cudaMemcpyHostToDevice)); }
+static void kv_h2d(__half * dst, const float * src, size_t n) {
+    std::vector<__half> h(n);
+    for (size_t i = 0; i < n; i++) h[i] = __float2half_rn(src[i]);
+    B200_CUDA_CHECK(cudaMemcpy(dst, h.data(), n * 2, cudaMemcpyHostToDevice));
 }
 
 template <typename E>
@@ -245,7 +254,6 @@ b200_falcon * b200_falcon_create_kv(const b200_falcon_params * p, int kv_ggml_ty
     if (kv_ggml_type != T_F32 && kv_ggml_type != T_F16) return nullptr;
     b200_falcon * f = new b200_falcon();
     f->hp = *p;
-    f->kv_type = kv_ggml_type;
     B200_ASSERT(p->n_embd % p->n_head == 0 && p->n_head % p->n_head_kv == 0);
     f->E = p->n_embd; f->H = p->n_head; f->HKV = p->n_head_kv; f->D = p->n_embd / p->n_head;
     f->QKV = (f->H + 2 * f->HKV) * f->D; f->FF = 4 * f->E; f->V = p->n_vocab;
@@ -265,15 +273,16 @@ b200_falcon * b200_falcon_create_kv(const b200_falcon_params * p, int kv_ggml_ty
         const size_t sb = (size_t) f->NL * f->shadow_layer * sizeof(__half);
         B200_CUDA_CHECK(cudaMalloc(d, sb ? sb : 4)); B200_CUDA_CHECK(cudaMemset(*d, 0, sb));
     };
-    if (f->kv_type == T_F16) {                   // the cache is the fp16 K plane and V rows (rows padded to a multiple of 64 like the planes)
-        f->shadow_layer = (size_t) attention_ctx_pad(p->n_ctx) * kv_row(f);
-        alloc16(&f->k16); alloc16(&f->v16);
-        if (shadow) alloc16(&f->vt16);
+    f->kv.ctx_pad = attention_ctx_pad(p->n_ctx);
+    if (kv_ggml_type == T_F16) {                 // the cache is the fp16 K plane and V rows (rows padded to a multiple of 64 like the planes)
+        f->shadow_layer = (size_t) f->kv.ctx_pad * kv_row(f);
+        alloc16(&f->kv.k16); alloc16(&f->kv.v16);
+        if (shadow) alloc16(&f->kv.vt16);
     } else {
         const size_t kv = (size_t) f->NL * p->n_ctx * kv_row(f) * sizeof(float);
-        B200_CUDA_CHECK(cudaMalloc(&f->k_cache, kv ? kv : 4)); B200_CUDA_CHECK(cudaMalloc(&f->v_cache, kv ? kv : 4));
-        B200_CUDA_CHECK(cudaMemset(f->k_cache, 0, kv)); B200_CUDA_CHECK(cudaMemset(f->v_cache, 0, kv));
-        if (shadow) { f->shadow_layer = attention_shadow_halves(f->HKV, p->n_ctx); alloc16(&f->k16); alloc16(&f->vt16); }
+        B200_CUDA_CHECK(cudaMalloc(&f->kv.k, kv ? kv : 4)); B200_CUDA_CHECK(cudaMalloc(&f->kv.v, kv ? kv : 4));
+        B200_CUDA_CHECK(cudaMemset(f->kv.k, 0, kv)); B200_CUDA_CHECK(cudaMemset(f->kv.v, 0, kv));
+        if (shadow) { f->shadow_layer = attention_shadow_halves(f->HKV, p->n_ctx); alloc16(&f->kv.k16); alloc16(&f->kv.vt16); }
     }
     B200_CUDA_CHECK(cudaMalloc(&f->inp, NB * f->E * 4)); B200_CUDA_CHECK(cudaMalloc(&f->qkv, NB * f->QKV * 4));
     B200_CUDA_CHECK(cudaMalloc(&f->att, NB * f->E * 4)); B200_CUDA_CHECK(cudaMalloc(&f->ao, NB * f->E * 4));
@@ -520,7 +529,7 @@ void b200_falcon_free(b200_falcon * f) {
     for (auto & L : f->layers) { free_matrix(f, L.wqkv); free_matrix(f, L.wo); free_matrix(f, L.up); free_matrix(f, L.down);
         cudaFree(L.ln_attn_g); cudaFree(L.ln_attn_b); cudaFree(L.ln_mlp_g); cudaFree(L.ln_mlp_b); }
     free_matrix(f, f->tok_emb); free_matrix(f, f->lm_head);
-    cudaFree(f->lnf_g); cudaFree(f->lnf_b); cudaFree(f->k_cache); cudaFree(f->v_cache); cudaFree(f->k16); cudaFree(f->vt16); cudaFree(f->v16);
+    cudaFree(f->lnf_g); cudaFree(f->lnf_b); cudaFree(f->kv.k); cudaFree(f->kv.v); cudaFree(f->kv.k16); cudaFree(f->kv.v16); cudaFree(f->kv.vt16);
     cudaFree(f->inp); cudaFree(f->qkv); cudaFree(f->att); cudaFree(f->ao); cudaFree(f->up); cudaFree(f->dn); cudaFree(f->logits);
     f->attn_scratch.release(); cudaFree(f->actq_mem); cudaFree(f->gen_na); cudaFree(f->gen_nm); cudaFree(f->gen_mm); cudaFree(f->xh_a); cudaFree(f->xh_b); cudaFree(f->xh_m);
     cudaFree(f->tokens_dev); cudaFree(f->n_past_dev); cudaFree(f->q_ctr); cudaFree(f->attn_dec_scratch); cudaFree(f->tap.mem);
@@ -626,17 +635,15 @@ static AttnParams attn_params(const b200_falcon * f, int l, int N, int n_past, f
     AttnParams ap = { f->H, f->HKV, f->D, N, n_past, graph_mode ? f->n_past_dev : nullptr, f->hp.n_ctx, (int64_t) f->QKV };
     ap.long_ctx = graph_mode ? f->cur_tier : 0;
     ap.rope_theta_scale = theta_scale;
-    const KvLayer kv = kv_layer(f, l);
-    ap.k16 = kv.k16; ap.vt16 = kv.vt16; ap.v16 = kv.v16;
+    ap.kv = kv_layer(f, l);
     return ap;
 }
 // RoPE + KV append of layer l's new rows (:2229-2281), then the attention qkv -> att (:2285-2366).  Prompts run eagerly, on s_main
 // like their attention: a scratch that has to grow waits for the previous user.
 static void enqueue_attention(b200_falcon * f, int l, const AttnParams & ap, cudaStream_t st) {
-    const KvLayer kv = kv_layer(f, l);
     float * scratch = ap.n_tok > 1 ? (float *) f->attn_scratch.get(attention_scratch_bytes(ap), st) : f->attn_dec_scratch;
     bool rotated = true;
-    f->launches += launch_attention(f->qkv, kv.k, kv.v, f->att, f->E, ap, scratch, st, nullptr, &rotated);
+    f->launches += launch_attention(f->qkv, f->att, f->E, ap, scratch, st, nullptr, &rotated);
     if (f->tap.mem) f->tap.rotated[l] = rotated;
 }
 
@@ -1038,36 +1045,21 @@ static int generate_impl(b200_falcon * f, int32_t first_token, int n_past, int n
 // (falcon_copy_state_data / falcon_set_state_data, libfalcon.cpp:4313-4490: n_tokens x n_embd_kv floats per layer for K and V);
 // here the cache is device-resident [layer][n_ctx][n_head_kv][head_dim] f32 or fp16 and rows are copied straight out of / into HBM.  The
 // host rows are f32 for either engine: an fp16 cache's values are widened exactly on the way out and rounded (to nearest even) on the way in.
-static void kv16_d2h(float * dst, const __half * src, size_t n) {
-    std::vector<__half> h(n);
-    B200_CUDA_CHECK(cudaMemcpy(h.data(), src, n * 2, cudaMemcpyDeviceToHost));
-    for (size_t i = 0; i < n; i++) dst[i] = __half2float(h[i]);
-}
-static void kv16_h2d(__half * dst, const float * src, size_t n) {
-    std::vector<__half> h(n);
-    for (size_t i = 0; i < n; i++) h[i] = __float2half_rn(src[i]);
-    B200_CUDA_CHECK(cudaMemcpy(dst, h.data(), n * 2, cudaMemcpyHostToDevice));
-}
 int b200_falcon_kv_read(b200_falcon * f, int layer, int pos, int n, float * k_out, float * v_out) {
     if (layer < f->hp.layer_first || layer >= f->hp.layer_last || pos < 0 || n < 0 || pos + n > f->hp.n_ctx) return 1;
-    const KvLayer c = kv_layer(f, layer - f->hp.layer_first);
+    const KvCache c = kv_layer(f, layer - f->hp.layer_first);
     const size_t row = kv_row(f), o = (size_t) pos * row, cnt = (size_t) n * row;
     B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
-    if (f->kv_type == T_F16) {
-        if (k_out) kv16_d2h(k_out, c.k16 + o, cnt);
-        if (v_out) kv16_d2h(v_out, c.v16 + o, cnt);
-        return 0;
-    }
-    if (k_out) B200_CUDA_CHECK(cudaMemcpy(k_out, c.k + o, cnt * 4, cudaMemcpyDeviceToHost));
-    if (v_out) B200_CUDA_CHECK(cudaMemcpy(v_out, c.v + o, cnt * 4, cudaMemcpyDeviceToHost));
+    auto get = [&](float * dst, const auto * src) { if (dst) kv_d2h(dst, src + o, cnt); };
+    if (kv_f16(c)) { get(k_out, c.k16); get(v_out, c.v16); } else { get(k_out, c.k); get(v_out, c.v); }
     return 0;
 }
 // the fp16 planes the prompt kernel reads (attention_ws.cu), positions [pos, pos + n) of `layer`: k16_out [n][n_head_kv][head_dim] (an fp16
 // engine's K cache itself), vt16_out [n_head_kv][head_dim][n].  The range may reach attention_ctx_pad(n_ctx), so that the padding can be inspected.
 int b200_falcon_kv_shadow_read(b200_falcon * f, int layer, int pos, int n, uint16_t * k16_out, uint16_t * vt16_out) {
-    const int ctx_pad = attention_ctx_pad(f->hp.n_ctx);
-    if (!f->k16 || (vt16_out && !f->vt16) || layer < f->hp.layer_first || layer >= f->hp.layer_last || pos < 0 || n < 0 || pos + n > ctx_pad) return 1;
-    const KvLayer c = kv_layer(f, layer - f->hp.layer_first);
+    const int ctx_pad = f->kv.ctx_pad;
+    if (!f->kv.k16 || (vt16_out && !f->kv.vt16) || layer < f->hp.layer_first || layer >= f->hp.layer_last || pos < 0 || n < 0 || pos + n > ctx_pad) return 1;
+    const KvCache c = kv_layer(f, layer - f->hp.layer_first);
     const size_t row = kv_row(f);
     B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
     if (k16_out && n) B200_CUDA_CHECK(cudaMemcpy(k16_out, c.k16 + (size_t) pos * row, (size_t) n * row * 2, cudaMemcpyDeviceToHost));
@@ -1076,18 +1068,12 @@ int b200_falcon_kv_shadow_read(b200_falcon * f, int layer, int pos, int n, uint1
 }
 int b200_falcon_kv_write(b200_falcon * f, int layer, int pos, int n, const float * k_in, const float * v_in) {
     if (layer < f->hp.layer_first || layer >= f->hp.layer_last || pos < 0 || n < 0 || pos + n > f->hp.n_ctx) return 1;
-    const KvLayer c = kv_layer(f, layer - f->hp.layer_first);
+    const KvCache c = kv_layer(f, layer - f->hp.layer_first);
     const size_t row = kv_row(f), o = (size_t) pos * row, cnt = (size_t) n * row;
     B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
-    if (f->kv_type == T_F16) {
-        if (k_in) kv16_h2d(c.k16 + o, k_in, cnt);
-        if (v_in) kv16_h2d(c.v16 + o, v_in, cnt);
-        if (c.vt16) launch_kv_shadow_refresh(c.v16, c.vt16, f->HKV, f->hp.n_ctx, pos, n, f->s_main);
-    } else {
-        if (k_in) B200_CUDA_CHECK(cudaMemcpy(c.k + o, k_in, cnt * 4, cudaMemcpyHostToDevice));
-        if (v_in) B200_CUDA_CHECK(cudaMemcpy(c.v + o, v_in, cnt * 4, cudaMemcpyHostToDevice));
-        if (c.k16) launch_kv_shadow_refresh(c.k, c.v, c.k16, c.vt16, f->HKV, f->hp.n_ctx, pos, n, f->s_main);
-    }
+    auto put = [&](auto * dst, const float * src) { if (src) kv_h2d(dst + o, src, cnt); };
+    if (kv_f16(c)) { put(c.k16, k_in); put(c.v16, v_in); } else { put(c.k, k_in); put(c.v, v_in); }
+    launch_kv_shadow_refresh(c, f->HKV, pos, n, f->s_main);
     B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
     return 0;
 }
@@ -1097,17 +1083,12 @@ int b200_falcon_kv_fill_random(b200_falcon * f, int pos, int n, uint64_t seed) {
     if (pos < 0 || n < 0 || pos + n > f->hp.n_ctx) return 1;
     const size_t row = kv_row(f);
     for (int l = 0; l < f->NL; l++) {
-        const KvLayer c = kv_layer(f, l);
+        const KvCache c = kv_layer(f, l);
         const int64_t cnt = (int64_t) ((size_t) n * row);
-        if (f->kv_type == T_F16) {                                   // the same values, rounded to the cache's fp16
-            fill_kernel<<<296, 256, 0, f->s_main>>>(c.k16 + (size_t) pos * row, cnt, 0.f, 1.f, seed + 2 * l);
-            fill_kernel<<<296, 256, 0, f->s_main>>>(c.v16 + (size_t) pos * row, cnt, 0.f, 1.f, seed + 2 * l + 1);
-            if (c.vt16) launch_kv_shadow_refresh(c.v16, c.vt16, f->HKV, f->hp.n_ctx, pos, n, f->s_main);
-            continue;
-        }
-        fill_kernel<<<296, 256, 0, f->s_main>>>(c.k + (size_t) pos * row, cnt, 0.f, 1.f, seed + 2 * l);
-        fill_kernel<<<296, 256, 0, f->s_main>>>(c.v + (size_t) pos * row, cnt, 0.f, 1.f, seed + 2 * l + 1);
-        if (c.k16) launch_kv_shadow_refresh(c.k, c.v, c.k16, c.vt16, f->HKV, f->hp.n_ctx, pos, n, f->s_main);
+        auto fill = [&](auto * dst, uint64_t s) { fill_kernel<<<296, 256, 0, f->s_main>>>(dst + (size_t) pos * row, cnt, 0.f, 1.f, s); };
+        if (kv_f16(c)) { fill(c.k16, seed + 2 * l); fill(c.v16, seed + 2 * l + 1); }      // the same values, rounded to the cache's fp16
+        else { fill(c.k, seed + 2 * l); fill(c.v, seed + 2 * l + 1); }
+        launch_kv_shadow_refresh(c, f->HKV, pos, n, f->s_main);
     }
     B200_CUDA_CHECK(cudaGetLastError());
     B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
@@ -1217,10 +1198,10 @@ int b200_falcon_tap_read(const b200_falcon * f, int layer, const char * node, vo
     return 1;
 }
 
-int b200_falcon_kv_type(const b200_falcon * f) { return f->kv_type; }
+int b200_falcon_kv_type(const b200_falcon * f) { return kv_f16(f->kv) ? T_F16 : T_F32; }
 size_t b200_falcon_kv_device_bytes(const b200_falcon * f) {
-    const size_t planes16 = (f->k16 ? 1 : 0) + (f->vt16 ? 1 : 0) + (f->v16 ? 1 : 0);
-    return (f->k_cache ? 2 * (size_t) f->NL * f->hp.n_ctx * kv_row(f) * sizeof(float) : 0) + planes16 * f->NL * f->shadow_layer * sizeof(__half);
+    const size_t planes16 = (f->kv.k16 ? 1 : 0) + (f->kv.v16 ? 1 : 0) + (f->kv.vt16 ? 1 : 0);
+    return (f->kv.k ? 2 * (size_t) f->NL * f->hp.n_ctx * kv_row(f) * sizeof(float) : 0) + planes16 * f->NL * f->shadow_layer * sizeof(__half);
 }
 int b200_falcon_last_launches(const b200_falcon * f) { return f->launches; }
 float b200_falcon_last_ms(const b200_falcon * f) { return f->last_ms; }

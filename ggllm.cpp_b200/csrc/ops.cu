@@ -382,36 +382,33 @@ void launch_rope_neox(float * x, int n_tok, int n_head, int head_dim, int64_t to
 }
 
 // fused RoPE(Q) + RoPE(K) + K append + V append (libfalcon.cpp:2229-2281): one CTA per (token, head slot)
-__global__ void rope_kv_append_kernel(float * __restrict__ qkv, float * __restrict__ kc, float * __restrict__ vc, AttnParams p, float theta_scale) {
+__global__ void rope_kv_append_kernel(float * __restrict__ qkv, AttnParams p) {
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     const int t = blockIdx.y, slot = blockIdx.x, i = threadIdx.x, D = p.head_dim, half = D / 2;
     const int n_past = p.n_past_dev ? *p.n_past_dev : p.n_past;
     const int pos = n_past + t;
     float * v = qkv + (size_t) t * p.qkv_stride + (size_t) slot * D;             // slots: Q heads | K heads | V heads
-    if (slot < p.n_head + p.n_head_kv) rope_pair(v, half, i, pos, theta_scale);
+    if (slot < p.n_head + p.n_head_kv) rope_pair(v, half, i, pos, p.rope_theta_scale);
     if (slot >= p.n_head) {
         const bool is_k = slot < p.n_head + p.n_head_kv;
         const int kvh = slot - p.n_head - (is_k ? 0 : p.n_head_kv);
         const size_t o = ((size_t) pos * p.n_head_kv + kvh) * D;
-        if (is_k) { kv_put_k(kc, p.k16, o + i, v[i]); kv_put_k(kc, p.k16, o + i + half, v[i + half]); }
-        else {
-            const int cp = (p.n_ctx + 63) / 64 * 64;
-            kv_put_v(vc, p.v16, p.vt16, o + i, kvh, i, pos, cp, v[i]); kv_put_v(vc, p.v16, p.vt16, o + i + half, kvh, i + half, pos, cp, v[i + half]);
-        }
+        if (is_k) { kv_put_k(p.kv, o + i, v[i]); kv_put_k(p.kv, o + i + half, v[i + half]); }
+        else { kv_put_v(p.kv, o + i, kvh, i, pos, v[i]); kv_put_v(p.kv, o + i + half, kvh, i + half, pos, v[i + half]); }
     }
 }
 // The same work for a batch of tokens (prompt).  The single-token kernel above recomputes the 32 rotation angles of a position in every
 // one of its (n_head + 2 n_head_kv) x n_tok tiny CTAs and scatters V^T two bytes at a time (at 512 tokens
 // about as long as the attention itself).  Here one CTA per token computes its cos / sin once and walks the row coalesced, and the V^T shadow
 // is written by extra CTAs that transpose 64 tokens x 64 dims through shared memory (128-byte rows).  Same arithmetic, same bits.
-__global__ void __launch_bounds__(256) rope_kv_append_batch_kernel(float * __restrict__ qkv, float * __restrict__ kc, float * __restrict__ vc, AttnParams p, float theta_scale) {
+__global__ void __launch_bounds__(256) rope_kv_append_batch_kernel(float * __restrict__ qkv, AttnParams p) {
     const int D = p.head_dim, half = D / 2, H = p.n_head, HKV = p.n_head_kv, N = p.n_tok;
     const int n_past = p.n_past_dev ? *p.n_past_dev : p.n_past;
     if ((int) blockIdx.x < N) {
         __shared__ float cs[64], sn[64];
         const int t = blockIdx.x, pos = n_past + t;
         if ((int) threadIdx.x < half) {
-            const float theta = rope_theta(pos, threadIdx.x, theta_scale);
+            const float theta = rope_theta(pos, threadIdx.x, p.rope_theta_scale);
             cs[threadIdx.x] = cosf(theta); sn[threadIdx.x] = sinf(theta);
         }
         __syncthreads();
@@ -424,15 +421,14 @@ __global__ void __launch_bounds__(256) rope_kv_append_batch_kernel(float * __res
             v[i] = r0; v[i + half] = r1;
             if (slot >= H) {
                 const size_t o = ((size_t) pos * HKV + (slot - H)) * D;
-                kv_put_k(kc, p.k16, o + i, r0); kv_put_k(kc, p.k16, o + i + half, r1);
+                kv_put_k(p.kv, o + i, r0); kv_put_k(p.kv, o + i + half, r1);
             }
         }
         for (int idx = threadIdx.x; idx < HKV * D; idx += 256)         // V^T: the CTAs below
-            kv_put_v(vc, p.v16, nullptr, (size_t) pos * HKV * D + idx, 0, 0, 0, 0, row[(size_t) (H + HKV) * D + idx]);
-    } else if (p.vt16) {
+            kv_put_v_rows(p.kv, (size_t) pos * HKV * D + idx, row[(size_t) (H + HKV) * D + idx]);
+    } else if (p.kv.vt16) {
         __shared__ __half sm[64][66];
         const int tile = (int) blockIdx.x - N, tt = tile / HKV, kvh = tile % HKV;
-        const size_t cp = (size_t) ((p.n_ctx + 63) / 64 * 64);
         for (int idx = threadIdx.x; idx < 64 * 64; idx += 256) {
             const int tl = idx >> 6, d = idx & 63, t = tt * 64 + tl;
             sm[tl][d] = t < N ? __float2half_rn(qkv[(size_t) t * p.qkv_stride + (size_t) (H + HKV + kvh) * 64 + d]) : __float2half_rn(0.f);
@@ -440,23 +436,23 @@ __global__ void __launch_bounds__(256) rope_kv_append_batch_kernel(float * __res
         __syncthreads();
         for (int idx = threadIdx.x; idx < 64 * 64; idx += 256) {
             const int d = idx >> 6, tl = idx & 63, t = tt * 64 + tl;
-            if (t < N) p.vt16[((size_t) kvh * 64 + d) * cp + n_past + t] = sm[tl][d];
+            if (t < N) p.kv.vt16[((size_t) kvh * 64 + d) * p.kv.ctx_pad + n_past + t] = sm[tl][d];
         }
     }
 }
 
-void launch_rope_kv_append(float * qkv, float * k_cache, float * v_cache, const AttnParams & p, float theta_scale, cudaStream_t stream) {
+void launch_rope_kv_append(float * qkv, const AttnParams & p, cudaStream_t stream) {
     if (p.n_tok <= 0) return;
-    if (p.n_tok > 1 && p.head_dim <= 128 && (!p.vt16 || p.head_dim == 64)) {
-        const unsigned grid = (unsigned) (p.n_tok + (p.vt16 ? (p.n_tok + 63) / 64 * p.n_head_kv : 0));
-        rope_kv_append_batch_kernel<<<grid, 256, 0, stream>>>(qkv, k_cache, v_cache, p, theta_scale);
+    if (p.n_tok > 1 && p.head_dim <= 128 && (!p.kv.vt16 || p.head_dim == 64)) {
+        const unsigned grid = (unsigned) (p.n_tok + (p.kv.vt16 ? (p.n_tok + 63) / 64 * p.n_head_kv : 0));
+        rope_kv_append_batch_kernel<<<grid, 256, 0, stream>>>(qkv, p);
         B200_CUDA_CHECK(cudaGetLastError());
         return;
     }
     dim3 grid((unsigned) (p.n_head + 2 * p.n_head_kv), (unsigned) p.n_tok);
     static bool set = false;
     if (!set) { B200_CUDA_CHECK(cudaFuncSetAttribute(rope_kv_append_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, B200_CARVEOUT)); set = true; }
-    rope_kv_append_kernel<<<grid, p.head_dim / 2, 0, stream>>>(qkv, k_cache, v_cache, p, theta_scale);
+    rope_kv_append_kernel<<<grid, p.head_dim / 2, 0, stream>>>(qkv, p);
     B200_CUDA_CHECK(cudaGetLastError());
 }
 
