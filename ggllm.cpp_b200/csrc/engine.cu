@@ -1077,6 +1077,43 @@ int b200_falcon_kv_write(b200_falcon * f, int layer, int pos, int n, const float
     B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
     return 0;
 }
+// the reference's session-state layout (kernels.h).  The cache rows of a layer are [n_ctx][E]: K rows copy straight across, V rows
+// are [position][E] and the state's V is [E][position]
+static bool ref_kv_args(const b200_falcon * f, int n, const void * v, const RefKvLayout & L) {
+    return !kv_f16(f->kv) && n >= 0 && n <= f->hp.n_ctx && (!v || L.v_ld >= (size_t) n);
+}
+extern "C++" int falcon_ref_kv_export(b200_falcon * f, int n, float * k, float * v, const RefKvLayout & L) {
+    if (!ref_kv_args(f, n, v, L)) return 1;
+    const size_t E = kv_row(f), lay = (size_t) f->hp.n_ctx * E;
+    if (n > 0 && k) B200_CUDA_CHECK(cudaMemcpy2DAsync(k, L.k_layer * 4, f->kv.k, lay * 4, (size_t) n * E * 4, f->NL, cudaMemcpyDeviceToHost, f->s_main));
+    float * stage = nullptr;
+    if (n > 0 && v) B200_CUDA_CHECK(cudaMalloc(&stage, (size_t) n * E * 4));
+    for (int l = 0; stage && l < f->NL; l++) {
+        launch_transpose_f32(kv_layer(f, l).v, (int64_t) E, n, (int) E, stage, n, f->s_main);
+        B200_CUDA_CHECK(cudaMemcpy2DAsync(v + l * L.v_layer, L.v_ld * 4, stage, (size_t) n * 4, (size_t) n * 4, E, cudaMemcpyDeviceToHost, f->s_main));
+    }
+    B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
+    if (stage) B200_CUDA_CHECK(cudaFree(stage));
+    return 0;
+}
+extern "C++" int falcon_ref_kv_import(b200_falcon * f, int n, const float * k, const float * v, const RefKvLayout & L) {
+    if (!ref_kv_args(f, n, v, L)) return 1;
+    const size_t E = kv_row(f), lay = (size_t) f->hp.n_ctx * E;
+    if (n > 0 && k) B200_CUDA_CHECK(cudaMemcpy2DAsync(f->kv.k, lay * 4, k, L.k_layer * 4, (size_t) n * E * 4, f->NL, cudaMemcpyHostToDevice, f->s_main));
+    float * stage = nullptr;
+    if (n > 0 && v) B200_CUDA_CHECK(cudaMalloc(&stage, (size_t) n * E * 4));
+    for (int l = 0; l < f->NL && n > 0; l++) {
+        const KvCache c = kv_layer(f, l);
+        if (v) {
+            B200_CUDA_CHECK(cudaMemcpy2DAsync(stage, (size_t) n * 4, v + l * L.v_layer, L.v_ld * 4, (size_t) n * 4, E, cudaMemcpyHostToDevice, f->s_main));
+            launch_transpose_f32(stage, n, (int) E, n, c.v, (int64_t) E, f->s_main);
+        }
+        launch_kv_shadow_refresh(c, f->HKV, 0, n, f->s_main);
+    }
+    B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
+    if (stage) B200_CUDA_CHECK(cudaFree(stage));
+    return 0;
+}
 // random K / V rows generated on the device for positions [pos, pos + n) of every local layer: pre-fills a long context
 // for throughput runs (BASELINE config 5: decode at 8k context) without evaluating 8k tokens first
 int b200_falcon_kv_fill_random(b200_falcon * f, int pos, int n, uint64_t seed) {

@@ -118,18 +118,24 @@ void op_unary(int op, const abi::tensor * src0, const abi::tensor * src1, abi::t
 //   eval 2.. : GET_ROWS(tok_embeddings, embd) marks the start: the token ids are on the host there.  Every node is claimed without
 //     computing anything until the first ROPE node, whose src1 holds n_past and the rope context (ggml.c:6947-6952): the engine
 //     evaluates the whole graph there (one CUDA graph launch for N = 1); "result_lm_head" receives the logits.
-// Conditions: every layer's four matrices offloaded (n_gpu_layers >= n_layer), head_dim 64, first eval at n_past 0.  Otherwise the
-// per-node path stays in charge.  Under takeover the reference's HOST KV cache is not maintained (the cache lives in HBM; use
-// b200_falcon_kv_read for session files).  B200_NO_TAKEOVER=1 disables it.
+//   a first eval at n_past > 0 (a session restored before it, falcon_main.cpp:662-673 then skips its BOS warm-up): the engine is built
+//     the same way, imports positions [0, n_past) from the host cache that eval read (cache_k rows, V from the buffer its "V_new" view
+//     wrote, column stride n_past + N) and replays the eval's N tokens at n_past.
+// Conditions: every layer's four matrices offloaded (n_gpu_layers >= n_layer), head_dim 64.  Otherwise the per-node path stays in charge.
+// Under takeover the reference's HOST KV cache is not maintained (the cache lives in HBM).  Session state still is what the reference
+// expects: falcon_copy_state_data / falcon_set_state_data (libfalcon.cpp:4226-4470) copy the KV cache through ggml_cpy graphs over 3-D
+// views of cache_k and the current V buffer, and between evals this hook serves those copies from the device cache (tk_state_copy).
+// B200_NO_TAKEOVER=1 disables it.
 b200_falcon * b200_takeover_engine = nullptr;          // the engine behind the hook (tests read its counters)
 
 struct Takeover {
     enum State { OFF, LEARNING, READY, DISABLED } state = OFF;
     std::map<std::string, const abi::tensor *> named;   // GGCC name -> model tensor
-    const abi::tensor * emb = nullptr, * cache_k = nullptr;
+    const abi::tensor * emb = nullptr, * cache_k = nullptr, * v_new = nullptr;   // v_new: the V buffer the learning eval wrote
     std::vector<int32_t> tokens; int N = 0, n_past = -1, rope_ctx = 0;
     bool active = false, launched = false;              // this eval is being evaluated by the engine
     int valid_upto = 0, n_vocab = 0, n_batch = 0;
+    int n_layer = 0, n_ctx = 0, e_kv = 0;               // the engine's cache: e_kv = n_head_kv * 64 floats per position and layer
     float * logits = nullptr; size_t logits_floats = 0; // pinned
     long evals_taken = 0;                               // by this engine (the cumulative count for tests / bench is g_tk_total)
 } g_tk;
@@ -197,7 +203,61 @@ bool tk_build() {
     }
     if (!ok) { b200_falcon_free(f); return false; }
     b200_takeover_engine = f; g_tk.n_vocab = hp.n_vocab;
+    g_tk.n_layer = n_layer; g_tk.n_ctx = hp.n_ctx; g_tk.e_kv = hp.n_head_kv * 64;
     return true;
+}
+
+// ---- session state behind the engine.  falcon_copy_state_data / falcon_set_state_data build, per plane, a CPY between a host blob and a
+// VIEW of the host cache (E = n_head_kv * 64, n = kv_ntok, offset 0):
+//   K: view of cache_k,                 ne (E, n, n_layer), nb (4, 4 E, 4 E n_ctx)  <->  blob [n_layer][n][E]
+//   V: view of cache_v_a or cache_v_b,  ne (n, E, n_layer), nb (4, 4 n, 4 E n_ctx)  <->  blob [n_layer][E][n]
+enum { KV_NONE, KV_K, KV_V };
+int kv_view_plane(const abi::tensor * t) {
+    if (!t || t->op != abi::OP_VIEW || !t->src0) return KV_NONE;
+    const char * n = t->src0->name;
+    if (strcmp(n, "cache_k") == 0) return KV_K;
+    // cache_v: the V cache of a FALCON_NO_KV_UPGRADE build, whose layout state_view_ntok refuses
+    return (strcmp(n, "cache_v_a") == 0 || strcmp(n, "cache_v_b") == 0 || strcmp(n, "cache_v") == 0) ? KV_V : KV_NONE;
+}
+// n if `view` has the state layout of `plane` over the engine's cache, else -1
+int state_view_ntok(const abi::tensor * view, int plane) {
+    const int64_t E = g_tk.e_kv, n = plane == KV_K ? view->ne[1] : view->ne[0];
+    const bool dims = plane == KV_K ? view->ne[0] == E && view->nb[1] == (size_t) E * 4 : view->ne[1] == E && view->nb[1] == (size_t) n * 4;
+    const bool ok = dims && view->type == T_F32 && view->data == view->src0->data && view->ne[2] == g_tk.n_layer && view->ne[3] == 1 &&
+                    view->nb[0] == 4 && view->nb[2] == (size_t) E * g_tk.n_ctx * 4 && n >= 0 && n <= g_tk.n_ctx;
+    return ok ? (int) n : -1;
+}
+// READY, no eval in flight: a CPY out of a view of the host cache is a save and is served from the device (claimed); a CPY into one is a
+// restore, which the CPU performs as well, so that the host state stays what the reference expects
+bool tk_state_copy(bool lead, abi::tensor * t) {
+    if (t->op != abi::OP_CPY) return false;
+    const int out = kv_view_plane(t->src0), in = kv_view_plane(t->src1);
+    if (out == KV_NONE && in == KV_NONE) return false;
+    if (!lead) return out != KV_NONE;
+    const abi::tensor * view = out != KV_NONE ? t->src0 : t->src1, * host = out != KV_NONE ? t : t->src0;
+    const int plane = out != KV_NONE ? out : in, n = state_view_ntok(view, plane);
+    if (n < 0 || !contiguous_f32(host) || nelements(host) != nelements(view)) {
+        fprintf(stderr, "b200: a copy %s the host KV cache ('%s') in a layout the device KV cache cannot serve; set B200_NO_TAKEOVER=1 to keep "
+                        "the per-node path\n", out != KV_NONE ? "out of" : "into", t->name);
+        abort();
+    }
+    const RefKvLayout L{ (size_t) n * g_tk.e_kv, (size_t) n, (size_t) n * g_tk.e_kv };
+    float * blob = (float *) host->data;
+    if (out != KV_NONE) {
+        if (n > g_tk.valid_upto) {
+            fprintf(stderr, "b200: session state of %d positions requested but the device KV cache holds %d\n", n, g_tk.valid_upto);
+            abort();
+        }
+        if (falcon_ref_kv_export(b200_takeover_engine, n, plane == KV_K ? blob : nullptr, plane == KV_V ? blob : nullptr, L) != 0) {
+            fprintf(stderr, "b200: KV state export failed (%d positions)\n", n); abort();
+        }
+        return true;
+    }
+    if (falcon_ref_kv_import(b200_takeover_engine, n, plane == KV_K ? blob : nullptr, plane == KV_V ? blob : nullptr, L) != 0) {
+        fprintf(stderr, "b200: KV state import failed (%d positions)\n", n); abort();
+    }
+    g_tk.valid_upto = n;
+    return false;
 }
 
 // returns true when the node is handled by the takeover machinery (the caller then returns true to ggml: skip the CPU)
@@ -227,15 +287,16 @@ bool tk_node(const abi::compute_params * params, abi::tensor * t) {
             tk_note(t->src0); tk_note(t->src1);
             if (t->op == abi::OP_ROPE && g_tk.n_past < 0) { g_tk.n_past = ((const int32_t *) t->src1->data)[0]; g_tk.rope_ctx = ((const int32_t *) t->src1->data)[3]; }
             if (t->op == abi::OP_VIEW && t->src0 && strcmp(t->src0->name, "cache_k") == 0) g_tk.cache_k = t->src0;
+            if (t->op == abi::OP_VIEW && t->src0 && strcmp(t->name, "V_new") == 0) g_tk.v_new = t->src0;        // libfalcon.cpp:2264-2271
         }
         return false;                                                          // the per-node path computes this eval
     }
-    if (!g_tk.active) return false;
+    if (!g_tk.active) return g_tk.state == Takeover::READY && tk_state_copy(lead, t);
     if (!lead) return true;
     if (t->op == abi::OP_ROPE && !g_tk.launched) {
         g_tk.n_past = ((const int32_t *) t->src1->data)[0]; g_tk.rope_ctx = ((const int32_t *) t->src1->data)[3];
         if (g_tk.n_past > g_tk.valid_upto) {
-            fprintf(stderr, "b200: eval at n_past %d but the device KV cache holds %d positions (KV state restored on the host?); "
+            fprintf(stderr, "b200: eval at n_past %d but the device KV cache holds %d positions; "
                             "set B200_NO_TAKEOVER=1 to keep the per-node path\n", g_tk.n_past, g_tk.valid_upto);
             abort();
         }
@@ -256,11 +317,16 @@ bool tk_node(const abi::compute_params * params, abi::tensor * t) {
 
 // called after the per-node path has finished the LAST node of the learning eval
 void tk_finish_learning() {
-    if (tk_build() && g_tk.n_past == 0) {
+    if (tk_build() && g_tk.n_past >= 0 && g_tk.N <= g_tk.n_batch) {
+        // positions before the eval (a restored session): the host cache this eval read, K rows and V as "V_new" left it
+        const size_t lay = (size_t) g_tk.n_ctx * g_tk.e_kv;
+        const bool imported = g_tk.n_past == 0 || (g_tk.v_new &&
+            falcon_ref_kv_import(b200_takeover_engine, g_tk.n_past, (const float *) g_tk.cache_k->data, (const float *) g_tk.v_new->data,
+                                 RefKvLayout{ lay, (size_t) (g_tk.n_past + g_tk.N), lay }) == 0);
         // replay the eval on the engine so that ITS cache holds these positions too (results discarded)
         float * lg = const_cast<float *>(tk_logits((size_t) g_tk.N * g_tk.n_vocab));
-        if (g_tk.N <= g_tk.n_batch && b200_falcon_eval(b200_takeover_engine, g_tk.tokens.data(), g_tk.N, 0, g_tk.rope_ctx, lg, 1) == 0) {
-            g_tk.valid_upto = g_tk.N; g_tk.state = Takeover::READY;
+        if (imported && b200_falcon_eval(b200_takeover_engine, g_tk.tokens.data(), g_tk.N, g_tk.n_past, g_tk.rope_ctx, lg, 1) == 0) {
+            g_tk.valid_upto = g_tk.n_past + g_tk.N; g_tk.state = Takeover::READY;
             if (getenv("B200_VERBOSE")) fprintf(stderr, "b200: Falcon eval graph recognised -- whole-graph evaluation on the device from the next eval on\n");
             return;
         }

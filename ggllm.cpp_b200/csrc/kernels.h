@@ -51,6 +51,8 @@ void   launch_add3(const float * a, const float * b, const float * c, float * y,
 void   launch_mul_bcast(const float * a, const float * b, float * y, int64_t n, int64_t nb, cudaStream_t stream);  // y[i] = a[i]*b[i%nb]
 void   launch_add_bcast(const float * a, const float * b, float * y, int64_t n, int64_t nb, cudaStream_t stream);
 void   launch_scale(const float * a, float s, float * y, int64_t n, cudaStream_t stream);
+// dst[c * ld_dst + r] = src[r * ld_src + c] for r < rows, c < cols (tiled through shared memory, coalesced on both sides)
+void   launch_transpose_f32(const float * src, int64_t ld_src, int rows, int cols, float * dst, int64_t ld_dst, cudaStream_t stream);
 struct RopeParams { int n_past; int head_dim; float theta_scale; };
 float  rope_theta_scale_host(int head_dim, int n_ctx_rope, int dynamic_mode, float ntk_alpha, int freq_base);
 float  falcon_rope_theta_scale(int head_dim, int n_ctx_rope, int n_ctx);   // Falcon's settings (libfalcon.cpp:2229-2234); n_ctx_rope 0: n_ctx
@@ -188,3 +190,11 @@ struct b200_falcon;
 bool   falcon_adopt_matrix(b200_falcon * f, const char * ggcc_name, const WPlanes & W);
 int    falcon_eval_begin(b200_falcon * f, const int32_t * tokens, int n_tokens, int n_past, int n_ctx_rope, int all_logits);   // enqueue only (b200_falcon_eval's checks and return codes)
 void   falcon_eval_finish(b200_falcon * f, float * logits);                                                                   // wait; logits (optional) receive what begin asked for
+// The KV section of the reference's session state (falcon_copy_state_data / falcon_set_state_data, libfalcon.cpp:4280-4330), host side:
+// positions [0, n) of every local layer in f32, K as n rows of n_head_kv * 64 floats, V transposed: n_head_kv * 64 columns of n positions,
+// column stride v_ld.  Local layer l's K starts k_layer floats after layer l - 1's, its V v_layer floats after.  Either plane may be null.
+// V goes through a device staging buffer and the tiled transpose; each byte crosses PCIe once.  Import also refreshes the fp16 shadow of
+// [0, n).  f32 caches only: returns 0, or 1 for an fp16 cache or n outside [0, n_ctx].
+struct RefKvLayout { size_t k_layer, v_ld, v_layer; };
+int    falcon_ref_kv_export(b200_falcon * f, int n, float * k, float * v, const RefKvLayout & L);
+int    falcon_ref_kv_import(b200_falcon * f, int n, const float * k, const float * v, const RefKvLayout & L);

@@ -350,6 +350,26 @@ void launch_mul_bcast(const float * a, const float * b, float * y, int64_t n, in
 void launch_add_bcast(const float * a, const float * b, float * y, int64_t n, int64_t nb, cudaStream_t s) { add_bcast_kernel<<<ew_grid(n), 256, 0, s>>>(a, b, y, n, nb); B200_CUDA_CHECK(cudaGetLastError()); }
 void launch_scale(const float * a, float sc, float * y, int64_t n, cudaStream_t s) { scale_kernel<<<ew_grid(n), 256, 0, s>>>(a, sc, y, n); B200_CUDA_CHECK(cudaGetLastError()); }
 
+// ---------------------------------------------------------------------------------------------- transpose
+// One CTA moves a 32 x 32 tile through shared memory: warp-wide reads along a source row, warp-wide writes along a destination row.
+// The padding column keeps the column-wise accesses to the tile free of bank conflicts.
+__global__ void __launch_bounds__(256) transpose_f32_kernel(const float * __restrict__ src, int64_t ld_src, int rows, int cols,
+                                                            float * __restrict__ dst, int64_t ld_dst) {
+    __shared__ float tile[32][33];
+    const int r0 = blockIdx.y * 32, c0 = blockIdx.x * 32, tx = threadIdx.x;
+    for (int i = threadIdx.y; i < 32; i += 8)
+        if (r0 + i < rows && c0 + tx < cols) tile[i][tx] = src[(int64_t) (r0 + i) * ld_src + c0 + tx];
+    __syncthreads();
+    for (int i = threadIdx.y; i < 32; i += 8)
+        if (c0 + i < cols && r0 + tx < rows) dst[(int64_t) (c0 + i) * ld_dst + r0 + tx] = tile[tx][i];
+}
+void launch_transpose_f32(const float * src, int64_t ld_src, int rows, int cols, float * dst, int64_t ld_dst, cudaStream_t s) {
+    if (rows <= 0 || cols <= 0) return;
+    B200_ASSERT((rows + 31) / 32 <= 65535);
+    transpose_f32_kernel<<<dim3((unsigned) ((cols + 31) / 32), (unsigned) ((rows + 31) / 32)), dim3(32, 8), 0, s>>>(src, ld_src, rows, cols, dst, ld_dst);
+    B200_CUDA_CHECK(cudaGetLastError());
+}
+
 // ---------------------------------------------------------------------------------------------- RoPE
 // theta_scale is computed on the host exactly as the CPU does (powf in fp32, ggml.c:12875-12898) and passed in.
 float rope_theta_scale_host(int head_dim, int n_ctx_rope, int dynamic_mode, float ntk_alpha, int freq_base) {
