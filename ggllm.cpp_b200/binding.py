@@ -26,7 +26,7 @@ PART_B = ["b200_falcon_create", "b200_falcon_create_kv", "b200_falcon_kv_type", 
           "b200_falcon_init_pipeline", "b200_falcon_eval", "b200_falcon_decode_dev", "b200_falcon_logits_dev", "b200_falcon_generate_greedy",
           "b200_falcon_last_launches", "b200_attention_long_launches", "b200_falcon_last_ms", "b200_falcon_stream", "b200_falcon_profile_matvec",
           "b200_falcon_kv_read", "b200_falcon_kv_write", "b200_falcon_kv_shadow_read", "b200_falcon_kv_fill_random", "b200_falcon_generate", "b200_falcon_generate_chain", "b200_falcon_load_seconds", "b200_falcon_save_kv", "b200_falcon_load_kv",
-          "b200_falcon_tap", "b200_falcon_tap_read", "b200_falcon_score", "b200_falcon_perplexity"]
+          "b200_falcon_tap", "b200_falcon_tap_read", "b200_falcon_score", "b200_falcon_perplexity", "b200_falcon_set_embeddings", "b200_falcon_embeddings"]
 
 
 def build(verbose=False):
@@ -88,6 +88,7 @@ def lib():
             "b200_falcon_tap": (i32, [vp, i32]), "b200_falcon_tap_read": (i32, [vp, i32, C.c_char_p, vp, sz]),
             "b200_token_nll": (None, [vp, i32, i32, i64, vp, vp, vp]),
             "b200_falcon_score": (i32, [vp, vp, i32, i32, i32, vp, vp]), "b200_falcon_perplexity": (i32, [vp, vp, i32, i32, vp, vp]),
+            "b200_falcon_set_embeddings": (i32, [vp, i32]), "b200_falcon_embeddings": (C.POINTER(C.c_float), [vp]),
         }
         for name, (res, args) in sig.items():
             fn = getattr(L, name)
@@ -394,6 +395,17 @@ class Falcon:
         if rc != 0:
             raise RuntimeError("b200_falcon_eval failed (rc=%d)" % rc)
         return out
+
+    def set_embeddings(self, on=True):
+        """falcon_context_params.embedding: every eval also returns the last token's final LayerNorm row (b200_falcon_set_embeddings)"""
+        if self.L.b200_falcon_set_embeddings(self.h, int(bool(on))) != 0:
+            raise RuntimeError("b200_falcon_set_embeddings: this rank has no head")
+
+    def embeddings(self):
+        """-> a copy of the n_embd floats of the most recent eval's "result_norm" row (falcon_get_embeddings), or None when embeddings
+        are off or the most recent eval call was not b200_falcon_eval"""
+        p = self.L.b200_falcon_embeddings(self.h)
+        return np.ctypeslib.as_array(p, (self.hp["n_embd"],)).copy() if p else None
 
     def score(self, tokens, n_past, targets, n_ctx_rope=0):
         """b200_falcon_score: evaluate `tokens` at n_past and return the terms -log p(targets[i]) as float32 [n_tokens], NaN where

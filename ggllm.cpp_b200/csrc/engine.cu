@@ -106,6 +106,11 @@ struct b200_falcon {
     size_t weight_bytes = 0;
     double load_seconds = 0.0; size_t load_bytes = 0;   // b200_falcon_load_ggcc
     size_t pending_floats = 0;                  // logits of the eval in flight (falcon_eval_begin / finish)
+    // falcon_context_params.embedding (b200_falcon_set_embeddings): the final LayerNorm's last head row ("result_norm") of every
+    // b200_falcon_eval goes to the pinned emb_h.  The fused head's LayerNorm kernel stores it in emb_dev, the generic head leaves it in
+    // gen_na; emb_src is the one the last head read.  emb_valid: emb_h holds the row of the most recent eval call.
+    bool emb_on = false, emb_valid = false;
+    float * emb_dev = nullptr, * emb_h = nullptr; const float * emb_src = nullptr;
     std::vector<const void *> borrowed;         // device planes adopted from another owner (ggml_cuda_transform_tensor): never freed here
     // test tap (b200_falcon_tap): while mem is set, every eval copies its intermediates into mem -- one slice of layer_bytes per local
     // layer at the end of that layer, then one slice after the head.  Node offsets are the same in every layer slice.
@@ -534,6 +539,7 @@ void b200_falcon_free(b200_falcon * f) {
     f->attn_scratch.release(); cudaFree(f->actq_mem); cudaFree(f->gen_na); cudaFree(f->gen_nm); cudaFree(f->gen_mm); cudaFree(f->xh_a); cudaFree(f->xh_b); cudaFree(f->xh_m);
     cudaFree(f->tokens_dev); cudaFree(f->n_past_dev); cudaFree(f->q_ctr); cudaFree(f->attn_dec_scratch); cudaFree(f->tap.mem);
     cudaFreeHost(f->tokens_h); cudaFreeHost(f->n_past_h); cudaFreeHost(f->logits_h);
+    cudaFree(f->emb_dev); cudaFreeHost(f->emb_h);
     cudaFree(f->score_tg); cudaFree(f->score_nll); cudaFreeHost(f->score_tg_h); cudaFreeHost(f->score_nll_h);
     for (auto & tier : f->graph) for (auto & g : tier) if (g.exec) cudaGraphExecDestroy(g.exec);
     cudaFree(f->tok_next); cudaFree(f->gen_hist); cudaFree(f->gen_step); cudaFree(f->sampler_work); sampler_state_free(f->sampler);
@@ -580,18 +586,26 @@ static void tap_head(b200_falcon * f, int N, int nr) {
 }
 
 // final LayerNorm + lm_head over rows x[0 .. nr) of the residual stream: libfalcon.cpp:2422-2440.  ra / rb (optional, quantised head
-// only): the last layer's branch outputs, which the LayerNorm kernel adds to x first (x = (ra + rb) + x, written back)
+// only): the last layer's branch outputs, which the LayerNorm kernel adds to x first (x = (ra + rb) + x, written back).  With embeddings
+// on, the quantised head's LayerNorm also stores its last row in fp32 (the row falcon_eval_internal copies, libfalcon.cpp:2551-2557).
 static void enqueue_head(b200_falcon * f, float * x, int nr, const float * ra, const float * rb, cudaStream_t sa) {
     const int E = f->E;
     if (f->generic_head) {
         launch_layernorm(x, E, f->lnf_g, f->lnf_b, f->gen_na, E, E, nr, sa); f->launches++;
         mm_any(f, f->lm_head, f->gen_na, nr, f->logits, f->V, false, sa);
+        f->emb_src = f->gen_na + (size_t) (nr - 1) * E;
         return;
     }
     ActQ xfr = f->xf; xfr.N = nr;
     if (nr > MMV_MAX_N) xfr.h = f->xh_a;
-    launch_layernorm_q(x, E, ra, rb, ra ? E : 0, f->lnf_g, f->lnf_b, &xfr, nullptr, nullptr, nullptr, E, nr, sa); f->launches++;
+    launch_layernorm_q(x, E, ra, rb, ra ? E : 0, f->lnf_g, f->lnf_b, &xfr, nullptr, nullptr, nullptr, E, nr, sa,
+                       f->emb_on ? f->emb_dev : nullptr, E, nr - 1); f->launches++;
     f->launches += launch_mul_mat_q(f->lm_head, xfr, nr, f->logits, f->V, EPI_NONE, sa);
+    f->emb_src = f->emb_dev;
+}
+// the head's "result_norm" row to the host, behind the logits copy of the same eval (a node of the G_HOST decode graph for one token)
+static void enqueue_embedding_copy(b200_falcon * f) {
+    if (f->emb_on) B200_CUDA_CHECK(cudaMemcpyAsync(f->emb_h, f->emb_src, (size_t) f->E * 4, cudaMemcpyDeviceToHost, f->s_main));
 }
 
 // Generation step (graph G_GEN): where the token id comes from and where the sampled one goes.
@@ -791,7 +805,10 @@ static void build_decode_graph(b200_falcon * f, int which, float theta_scale, in
     f->ring_mode = which == G_GEN;                 // (the eager pass above ran without it: every rank must issue the same NCCL calls there)
     enqueue_eval(f, 1, 0, theta_scale, true, 0);
     f->ring_mode = false;
-    if (which == G_HOST && f->last) B200_CUDA_CHECK(cudaMemcpyAsync(f->logits_h, f->logits, (size_t) f->V * 4, cudaMemcpyDeviceToHost, f->s_main));
+    if (which == G_HOST && f->last) {
+        B200_CUDA_CHECK(cudaMemcpyAsync(f->logits_h, f->logits, (size_t) f->V * 4, cudaMemcpyDeviceToHost, f->s_main));
+        enqueue_embedding_copy(f);
+    }
     B200_CUDA_CHECK(cudaStreamEndCapture(f->s_main, &g));
     B200_CUDA_CHECK(cudaGraphInstantiate(&dg.exec, g, 0));
     B200_CUDA_CHECK(cudaGraphDestroy(g));
@@ -865,14 +882,17 @@ extern "C++" int falcon_eval_begin(b200_falcon * f, const int32_t * tokens, int 
                 B200_CUDA_CHECK(cudaFreeHost(f->logits_h)); f->logits_h_floats = nfl; B200_CUDA_CHECK(cudaMallocHost(&f->logits_h, nfl * 4));
             }
             B200_CUDA_CHECK(cudaMemcpyAsync(f->logits_h, f->logits, nfl * 4, cudaMemcpyDeviceToHost, f->s_main));
+            enqueue_embedding_copy(f);
             f->pending_floats = nfl;
         }
     }
+    f->emb_valid = f->emb_on;
     return 0;
 }
-extern "C++" void falcon_eval_finish(b200_falcon * f, float * logits) {
+extern "C++" void falcon_eval_finish(b200_falcon * f, float * logits, float * embedding) {
     B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
     if (logits && f->pending_floats) memcpy(logits, f->logits_h, f->pending_floats * 4);
+    if (embedding) { B200_ASSERT(f->emb_valid); memcpy(embedding, f->emb_h, (size_t) f->E * 4); }
     B200_CUDA_CHECK(cudaEventElapsedTime(&f->last_ms, f->e_t0, f->e_t1));
 }
 int b200_falcon_eval(b200_falcon * f, const int32_t * tokens, int n_tokens, int n_past, int n_ctx_rope, float * logits, int all_logits) {
@@ -881,6 +901,18 @@ int b200_falcon_eval(b200_falcon * f, const int32_t * tokens, int n_tokens, int 
     falcon_eval_finish(f, logits);
     return 0;
 }
+
+int b200_falcon_set_embeddings(b200_falcon * f, int on) {
+    if (!f->last) return 1;
+    if ((on != 0) != f->emb_on) invalidate_graphs(f);          // the decode graphs hold the LayerNorm kernel's output and the copy, or neither
+    f->emb_on = on != 0;
+    if (f->emb_on && !f->emb_dev) {
+        B200_CUDA_CHECK(cudaMalloc(&f->emb_dev, (size_t) f->E * 4)); B200_CUDA_CHECK(cudaMallocHost(&f->emb_h, (size_t) f->E * 4));
+    }
+    if (!f->emb_on) f->emb_valid = false;
+    return 0;
+}
+const float * b200_falcon_embeddings(const b200_falcon * f) { return f->emb_valid ? f->emb_h : nullptr; }
 
 int b200_falcon_score(b200_falcon * f, const int32_t * tokens, int n_tokens, int n_past, int n_ctx_rope, const int32_t * targets, float * nll) {
     if (f->hp.world > 1) return 1;
@@ -893,6 +925,7 @@ int b200_falcon_score(b200_falcon * f, const int32_t * tokens, int n_tokens, int
         scored = scored || targets[i] >= 0;
     }
     if (scored && !nll) return 1;
+    f->emb_valid = false;
     const float theta = falcon_rope_theta_scale(f->D, n_ctx_rope, f->hp.n_ctx);
     const size_t bytes = (size_t) n_tokens * 4;
     memcpy(f->tokens_h, tokens, bytes); memcpy(f->score_tg_h, targets, bytes);
@@ -916,6 +949,7 @@ int b200_falcon_perplexity(b200_falcon * f, const int32_t * tokens, int n_tokens
     for (int i = 0; i < n_tokens; i++) if (tokens[i] < 0 || tokens[i] >= f->V) return -1;
     const int n_chunk = n_tokens / n_ctx;
     if (n_chunk == 0) return 0;
+    f->emb_valid = false;
     const int n_batch = f->hp.n_batch > 0 ? f->hp.n_batch : 1, first = std::min(512, n_ctx / 2);
     const size_t n_used = (size_t) n_chunk * n_ctx;
     std::vector<int32_t> tg(n_used, -1);
@@ -958,6 +992,7 @@ int b200_falcon_perplexity(b200_falcon * f, const int32_t * tokens, int n_tokens
 
 int b200_falcon_decode_dev(b200_falcon * f, const int32_t * token_dev, int n_past, int n_ctx_rope) {
     if (n_past < 0 || n_past >= f->hp.n_ctx) return 1;                       // the KV append would leave this layer's cache slice
+    f->emb_valid = false;
     const float theta = falcon_rope_theta_scale(f->D, n_ctx_rope, f->hp.n_ctx);
     const int tier = tier_of(n_past);
     // position and token id are device scalars the graph (and a build's eager pass) reads; both are set stream-ordered (the position
@@ -1015,6 +1050,7 @@ int b200_falcon_generate(b200_falcon * f, const b200_sampling_params * sp, const
 }
 static int generate_impl(b200_falcon * f, int32_t first_token, int n_past, int n_steps, int n_ctx_rope, int32_t * tokens_out) {
     if (n_steps <= 0 || n_past < 0 || n_past + n_steps > f->hp.n_ctx || first_token < 0 || first_token >= f->V) return 1;
+    f->emb_valid = false;
     const float theta = falcon_rope_theta_scale(f->D, n_ctx_rope, f->hp.n_ctx);
     cudaStream_t st = f->s_main;
     set_i32_kernel<<<1, 1, 0, st>>>(f->n_past_dev, n_past);

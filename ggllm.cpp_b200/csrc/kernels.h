@@ -39,10 +39,12 @@ bool   mmv_fast_fills_sm(const WPlanes & W);       // its CTAs leave no register
 // ---- ops.cu
 void   launch_layernorm(const float * x, int64_t x_stride, const float * g, const float * b, float * y, int64_t y_stride,
                         int n, int rows, cudaStream_t stream);              // y = norm(x)*g + b ; g,b may be null (plain ggml_norm)
-// [x = (ra + rb) + x, written back] ; A1 = Q(norm(x)*g1+b1) ; A2 = Q(norm(x)*g2+b2) (optional)
+// [x = (ra + rb) + x, written back] ; A1 = Q(norm(x)*g1+b1) ; A2 = Q(norm(x)*g2+b2) (optional) ; with y: rows r >= y_row0 also
+// store norm(x)*g1+b1 in fp32 at y + (r - y_row0) * y_stride (16-byte aligned rows)
 void   launch_layernorm_q(float * x, int64_t x_stride, const float * ra, const float * rb, int64_t r_stride,
                           const float * g1, const float * b1, const ActQ * A1,
-                          const float * g2, const float * b2, const ActQ * A2, int n, int rows, cudaStream_t stream);
+                          const float * g2, const float * b2, const ActQ * A2, int n, int rows, cudaStream_t stream,
+                          float * y = nullptr, int64_t y_stride = 0, int y_row0 = 0);
 void   launch_argmax_hist(const float * x, int n, int32_t * out, int32_t * hist, int * step, cudaStream_t stream);  // greedy: lowest index on ties; hist[(*step)++] = id (graph-replayable)
 void   launch_gelu(const float * x, float * y, int64_t n, cudaStream_t stream);
 void   launch_f32_to_f16(const float * x, __half * y, int64_t n, cudaStream_t stream);     // the fp16 activation rows of an F16-weight mat-mul
@@ -189,7 +191,7 @@ void   launch_token_nll(const float * logits, int n_vocab, int n_rows, int64_t r
 struct b200_falcon;
 bool   falcon_adopt_matrix(b200_falcon * f, const char * ggcc_name, const WPlanes & W);
 int    falcon_eval_begin(b200_falcon * f, const int32_t * tokens, int n_tokens, int n_past, int n_ctx_rope, int all_logits);   // enqueue only (b200_falcon_eval's checks and return codes)
-void   falcon_eval_finish(b200_falcon * f, float * logits);                                                                   // wait; logits (optional) receive what begin asked for
+void   falcon_eval_finish(b200_falcon * f, float * logits, float * embedding = nullptr);    // wait; logits (optional) receive what begin asked for, embedding (optional, embeddings on) the n_embd floats of b200_falcon_embeddings
 // The KV section of the reference's session state (falcon_copy_state_data / falcon_set_state_data, libfalcon.cpp:4280-4330), host side:
 // positions [0, n) of every local layer in f32, K as n rows of n_head_kv * 64 floats, V transposed: n_head_kv * 64 columns of n positions,
 // column stride v_ld.  Local layer l's K starts k_layer floats after layer l - 1's, its V v_layer floats after.  Either plane may be null.

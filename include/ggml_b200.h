@@ -260,6 +260,14 @@ void          b200_falcon_init_pipeline(b200_falcon * f, const void * id128);
  * In a pipeline every rank calls it; only the last rank's `logits` are written.  Returns 0 on success. */
 int           b200_falcon_eval(b200_falcon * f, const int32_t * tokens, int n_tokens, int n_past, int n_ctx_rope,
                                float * logits, int all_logits);
+/* falcon_context_params.embedding (libfalcon.h:108): with it on, every b200_falcon_eval also brings the last token's row of the final
+ * LayerNorm ("result_norm", libfalcon.cpp:2422-2431) to the host, in the same synchronise as its logits; the row is exactly the fp32
+ * values the head quantises for lm_head.  Off by default, and off changes nothing.  Returns 0, or 1 on a rank without the head. */
+int           b200_falcon_set_embeddings(b200_falcon * f, int on);
+/* falcon_get_embeddings (libfalcon.h:267): n_embd floats, the row of the most recent b200_falcon_eval; NULL with embeddings off, before
+ * any eval and after any other eval call (b200_falcon_score / _perplexity / _decode_dev / _generate*, which do not produce it).  The
+ * buffer is the engine's and is overwritten by the next eval. */
+const float * b200_falcon_embeddings(const b200_falcon * f);
 /* b200_falcon_eval that scores its rows on the device instead of returning logits (single GPU): targets[i] in [0, n_vocab) scores
  * row i -- nll[i] (host) receives b200_token_nll's term for it -- and -1 skips it (nll[i] untouched).  No logits cross PCIe.
  * A batch with a scored row runs the final LayerNorm and lm_head over all n_tokens rows, exactly as b200_falcon_eval(all_logits = 1)
