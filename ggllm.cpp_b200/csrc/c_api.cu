@@ -137,6 +137,12 @@ int b200_mul_mat_vec_q_chain(const b200_weight * w, const b200_actq * a_in, floa
     return launch_mmv_fast(W, a_in->A, y, W.M, e, g_stream) ? 1 : 0;
 }
 
+int b200_gemm_launch_shape(int wtype, int64_t K, int64_t M, int N, int64_t x_stride, int epilogue_gelu, int * out) {
+    const GemmTcShape s = gemm_tc_pick_shape(wtype, K, M, N, x_stride, true, epilogue_gelu);
+    if (out) { out[0] = s.bn; out[1] = s.ksplit; out[2] = s.producer; }
+    return s.bn ? 1 : 0;
+}
+
 int b200_mul_mat_f16(const b200_weight * w, const void * x_f16, int64_t x_stride, int N, float * y, int64_t y_stride, int epi_gelu, int impl) {
     if (impl == 0) { launch_gemm_simt(w->W, (const __half *) x_f16, x_stride, N, y, y_stride, epi_gelu, g_stream); return 1; }
     return launch_gemm_tc(w->W, (const __half *) x_f16, x_stride, N, y, y_stride, epi_gelu, g_stream) ? 1 : 0;

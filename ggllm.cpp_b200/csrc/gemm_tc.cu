@@ -323,8 +323,8 @@ void launch_typed(const CUtensorMap & map, const GemmArgs & a, cudaStream_t stre
 }
 
 template <int BN>
-void launch_bn(const CUtensorMap & map, const GemmArgs & a, cudaStream_t stream) {
-    switch (a.W.type) {
+void launch_bn(int producer, const CUtensorMap & map, const GemmArgs & a, cudaStream_t stream) {
+    switch (producer) {
         case T_Q4_K: launch_typed<T_Q4_K, BN>(map, a, stream); break;
         case T_Q4_0: launch_typed<T_Q4_0, BN>(map, a, stream); break;
         case T_Q3_K: launch_typed<T_Q3_K, BN>(map, a, stream); break;
@@ -334,15 +334,24 @@ void launch_bn(const CUtensorMap & map, const GemmArgs & a, cudaStream_t stream)
 
 } // namespace
 
+GemmTcShape gemm_tc_pick_shape(int type, int64_t K, int64_t M, int N, int64_t x_stride, bool x_aligned, int epi_gelu) {
+    if (N < 1 || N > N_MAX || K % BK != 0 || (x_stride % 8) != 0 || !x_aligned) return {};
+    GemmTcShape s;
+    s.bn = N <= 64 ? 64 : N <= 128 ? 128 : 256;
+    // fewer than ~100 tiles cannot fill the 132 SMs of an H100: split K in two (deterministic, see GemmArgs::ksplit)
+    const int64_t tiles = (M + BM - 1) / BM * ((N + s.bn - 1) / s.bn);
+    s.ksplit = (tiles < 100 && !epi_gelu && K / BK >= 8) ? 2 : 1;
+    s.producer = (type == T_Q4_K || type == T_Q4_0 || type == T_Q3_K) ? type : -1;
+    return s;
+}
+
 // X: fp16 [N][x_stride] (x_stride >= K, multiple of 8), Y: fp32 [N][y_stride].  N <= 512, K % 64 == 0.
 bool launch_gemm_tc(const WPlanes & W, const __half * X, int64_t x_stride, int N, float * Y, int64_t y_stride, int epi_gelu, cudaStream_t stream) {
-    if (N > N_MAX || W.K % BK != 0 || (x_stride % 8) != 0 || ((uintptr_t) X & 15) != 0) return false;
+    const GemmTcShape s = gemm_tc_pick_shape(W.type, W.K, W.M, N, x_stride, ((uintptr_t) X & 15) == 0, epi_gelu);
+    if (!s.bn) return false;
     GemmArgs a;
-    a.W = W; a.Y = Y; a.y_stride = y_stride; a.N = N; a.epi_gelu = epi_gelu;
-    const int BN = N <= 64 ? 64 : N <= 128 ? 128 : 256;
-    // fewer than ~100 tiles cannot fill the 132 SMs of an H100: split K in two (deterministic, see GemmArgs::ksplit)
-    const int tiles = (W.M + BM - 1) / BM * ((N + BN - 1) / BN);
-    a.ksplit = (tiles < 100 && !epi_gelu && W.K / BK >= 8) ? 2 : 1;
+    a.W = W; a.Y = Y; a.y_stride = y_stride; a.N = N; a.epi_gelu = epi_gelu; a.ksplit = s.ksplit;
+    const int BN = s.bn;
     // the two halves add into Y: clear the N rows of M outputs, and only those (columns M .. y_stride-1 belong to the caller)
     if (a.ksplit > 1) B200_CUDA_CHECK(cudaMemset2DAsync(Y, (size_t) y_stride * sizeof(float), 0, (size_t) W.M * sizeof(float), (size_t) N, stream));
     CUtensorMap map;
@@ -353,8 +362,8 @@ bool launch_gemm_tc(const WPlanes & W, const __half * X, int64_t x_stride, int N
     const CUresult rc = get_encode()(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void *) X, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (rc != CUDA_SUCCESS) { fprintf(stderr, "b200: cuTensorMapEncodeTiled failed (%d)\n", (int) rc); exit(1); }
-    if (BN == 64) launch_bn<64>(map, a, stream);
-    else if (BN == 128) launch_bn<128>(map, a, stream);
-    else launch_bn<256>(map, a, stream);
+    if (BN == 64) launch_bn<64>(s.producer, map, a, stream);
+    else if (BN == 128) launch_bn<128>(s.producer, map, a, stream);
+    else launch_bn<256>(s.producer, map, a, stream);
     return true;
 }

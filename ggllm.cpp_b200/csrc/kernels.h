@@ -160,6 +160,11 @@ size_t mul_mat_scratch_bytes(const WPlanes & W, int N);
 void   launch_mmq_gemm(const WPlanes & W, const __half * X, int64_t x_stride, int N, float * Y, int64_t y_stride, int epi_gelu, cudaStream_t stream);
 void   launch_gemm_simt(const WPlanes & W, const __half * X, int64_t x_stride, int N, float * Y, int64_t y_stride, int epi_gelu, cudaStream_t stream);
 bool   launch_gemm_tc(const WPlanes & W, const __half * X, int64_t x_stride, int N, float * Y, int64_t y_stride, int epi_gelu, cudaStream_t stream);   // false: shape not covered
+// what launch_gemm_tc launches: bn token-tile width (64 / 128 / 256), ksplit CTAs over K (1 / 2), producer the fast dequantiser's
+// type (T_Q4_K, T_Q4_0, T_Q3_K) or -1 for the generic one; bn == 0: not covered (N outside 1..512, K % 64, x_stride % 8, X not
+// 16-byte aligned), nothing launched
+struct GemmTcShape { int bn, ksplit, producer; };
+GemmTcShape gemm_tc_pick_shape(int type, int64_t K, int64_t M, int N, int64_t x_stride, bool x_aligned, int epi_gelu);
 
 // ---- sampling.cu: falcon_main's sampling chain on the device (logit bias, repetition / frequency / presence penalties, top-k,
 // tail-free, typical, top-p, temperature, mirostat 1 / 2, MT19937 draw)

@@ -107,10 +107,17 @@ int    b200_mmv_max_n(void);
  * when the generic ring kernel runs.  B200_MMV_GENERIC is not applied here. */
 int    b200_mmv_launch_shape(int ggml_type, int64_t K, int * nt_j_d);
 /* the GEMM half alone, on fp16 activations x[n][k] already on the device (what b200_mul_mat does after quantising):
- * impl 1 = wgmma tensor-core kernel (returns 0 if the shape is not covered: N > 512 or K % 64 != 0),
+ * impl 1 = wgmma tensor-core kernel (returns 0 and writes nothing if the shape is not covered: see b200_gemm_launch_shape, and x_f16_dev
+ *          must be 16-byte aligned),
  * impl 0 = CUDA-core kernel with identical operand rounding (the test reference for impl 1). */
 int    b200_mul_mat_f16(const b200_weight * w, const void * x_f16_dev, int64_t x_stride, int N, float * y_dev, int64_t y_stride,
                         int epilogue_gelu, int impl);
+/* which kernel b200_mul_mat_f16(impl 1) runs for a weight type, M rows of K weights, N tokens x_stride halves apart and an epilogue,
+ * on a 16-byte aligned x (b200_mul_mat runs the same choice on each chunk of at most 512 tokens).  Host only, no device needed.
+ * Returns 1 and out = {token-tile width BN (64, 128 or 256), K split over 1 or 2 CTAs, producer} for the wgmma kernel, where the
+ * producer is the weight type of a dedicated dequantiser (GGML_TYPE_Q4_K, Q4_0 or Q3_K) or -1 for the generic one; 0 (out = {0, 0, 0})
+ * when the shape is not covered (N outside 1..512, K % 64 != 0, x_stride % 8 != 0) and the CUDA-core kernel runs. */
+int    b200_gemm_launch_shape(int ggml_type, int64_t K, int64_t M, int N, int64_t x_stride, int epilogue_gelu, int * out);
 
 /* ---- the other operators of the Falcon graph, CPU-oracle numerics (SURVEY.md section 9.2) */
 /* y = norm(x) * g + b per row of n values (g, b may be NULL = plain ggml_norm, ggml.c:10540-10599) */

@@ -268,25 +268,6 @@ def test_tensor_core_gemm_matches_cuda_core_gemm(gpu, orc, t, M, K, N, gelu):
     assert np.all(np.abs(a - exact) <= budget), float(np.abs(a - exact).max())
 
 
-@pytest.mark.parametrize("t", [po.Q4_K, po.Q4_0, po.Q3_K, po.Q6_K, po.Q5_0])
-@pytest.mark.parametrize("N", [512, 200])
-def test_tensor_core_gemm_operand_is_the_exact_fp16_weight(gpu, orc, t, N):
-    """One-hot activation rows read the dequantised A operand back through the tensor cores: Y[n][m] = fp16(w[m][k_n]) exactly.
-    Pins the per-type dequantisation producers of gemm_tc.cu (Q4_K fp32 fma; Q4_0 / Q3_K half arithmetic; generic for the rest),
-    with one token tile (N = 200) and two (N = 512), to dequantize_row_* + one fp16 rounding."""
-    M, K = 300, 1024
-    wq = _weights(orc, t, M, K, seed=11)
-    W = gpu.Weight(t, K, M, wq)
-    want = orc.dequantize(t, wq, K).astype(np.float16).astype(np.float32)          # [M][K]
-    for off in range(0, K, N):
-        cols = (off + np.arange(N)) % K
-        xh = np.zeros((N, K), np.float16); xh[np.arange(N), cols] = 1.0
-        xd, yd = gpu.DevBuf(src=xh), gpu.DevBuf(N * M * 4)
-        assert gpu.lib().b200_mul_mat_f16(W.h, xd.ptr, K, N, yd.ptr, M, 0, 0) == 1
-        got = yd.download(np.float32, (N, M))
-        assert np.array_equal(got, want[:, cols].T), (t, N, off)
-
-
 @pytest.mark.parametrize("t,K,M", [(po.Q4_K, 8192, 32768), (po.Q4_K, 512, 768), (po.Q4_0, 4544, 18176)])
 def test_matvec_chain_quantises_output_for_next_matmul(gpu, orc, t, K, M):
     """ffn_up -> ffn_down hand-over: the mat-vec's own CTAs quantise the (GELU'd) output row, 256 values at a time, as
