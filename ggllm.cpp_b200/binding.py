@@ -17,7 +17,7 @@ PART_A = ["b200_event_create", "b200_event_destroy", "b200_event_record", "b200_
           "b200_stream_synchronize", "b200_init", "b200_device_count", "b200_set_stream", "b200_synchronize", "b200_malloc", "b200_free", "b200_memcpy_h2d",
           "b200_memcpy_d2h", "b200_memset", "b200_host_malloc", "b200_host_free", "b200_weight_upload", "b200_weight_random",
           "b200_weight_free", "b200_weight_device_bytes", "b200_dequantize_rows", "b200_actq_alloc", "b200_actq_free",
-          "b200_quantize_act", "b200_actq_download", "b200_actq_alloc_f16", "b200_actq_download_f16", "b200_actq_to_f16", "b200_mul_mat", "b200_mul_mat_f16", "b200_mul_mat_vec_q", "b200_mul_mat_vec_q_chain", "b200_quantize_weights", "b200_mmv_max_n", "b200_mmv_launch_shape", "b200_gemm_launch_shape", "b200_layernorm",
+          "b200_quantize_act", "b200_actq_download", "b200_actq_alloc_f16", "b200_actq_download_f16", "b200_actq_to_f16", "b200_mul_mat", "b200_mul_mat_f16", "b200_mul_mat_vec_q", "b200_mul_mat_vec_q_chain", "b200_quantize_weights", "b200_quantize_weights_rows", "b200_mmv_max_n", "b200_mmv_launch_shape", "b200_gemm_launch_shape", "b200_layernorm",
           "b200_gelu", "b200_add", "b200_rope_neox", "b200_attention", "b200_layernorm_q", "b200_attention_decode", "b200_attention_kv16", "b200_attention_decode_kv16",
           "b200_sampler_create", "b200_sampler_create_chain", "b200_sampler_sample", "b200_sampler_mirostat_mu", "b200_sampler_free",
           "b200_sampler_tap", "b200_sampler_tap_read", "b200_token_nll"]
@@ -58,7 +58,7 @@ def lib():
             "b200_actq_download": (None, [vp, vp, vp, vp, vp]),
             "b200_actq_alloc_f16": (vp, [i32, i64, i32]), "b200_actq_download_f16": (None, [vp, vp]), "b200_actq_to_f16": (None, [vp, vp, i64]),
             "b200_mul_mat": (None, [vp, vp, i64, i32, vp, i64]), "b200_mul_mat_vec_q": (None, [vp, vp, vp, i64, i32, vp, vp]),
-            "b200_mmv_max_n": (i32, []), "b200_mmv_launch_shape": (i32, [i32, i64, vp]), "b200_gemm_launch_shape": (i32, [i32, i64, i64, i32, i64, i32, vp]),"b200_mul_mat_vec_q_chain": (i32, [vp, vp, vp, i32, vp]), "b200_quantize_weights": (i32, [i32, vp, vp, i64]), "b200_mul_mat_f16": (i32, [vp, vp, i64, i32, vp, i64, i32, i32]),
+            "b200_mmv_max_n": (i32, []), "b200_mmv_launch_shape": (i32, [i32, i64, vp]), "b200_gemm_launch_shape": (i32, [i32, i64, i64, i32, i64, i32, vp]),"b200_mul_mat_vec_q_chain": (i32, [vp, vp, vp, i32, vp]), "b200_quantize_weights": (i32, [i32, vp, vp, i64]), "b200_quantize_weights_rows": (i32, [i32, vp, vp, i64, i64]), "b200_mul_mat_f16": (i32, [vp, vp, i64, i32, vp, i64, i32, i32]),
             "b200_layernorm": (None, [vp, i64, vp, vp, vp, i64, i32, i32]), "b200_gelu": (None, [vp, vp, i64]), "b200_add": (None, [vp, vp, vp, i64]),
             "b200_rope_neox": (None, [vp, i32, i32, i32, i64, i32, i32, i32, f32, i32]),
             "b200_attention": (None, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32]),

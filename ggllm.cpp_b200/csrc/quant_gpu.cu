@@ -2,14 +2,14 @@
 // (SURVEY section 8f-3, first two types: the ones BASELINE's models use).
 //   Q4_0: quantize_row_q4_0_reference, ggml.c:927-962
 //   Q4_K: quantize_row_q4_K_reference, k_quants.c:542-605, with make_qkx1_quants (:222-262) and nearest_int (:50-55)
-// One thread per block, the block's arithmetic in the CPU's order with explicitly rounded fp32 operations (no FMA
+// Q4_0: one thread per block.  Q4_K: one thread per row, walking its blocks in order (make_qkx1_quants carries codes from block
+// to block, see quantize_q4_K_kernel).  The arithmetic is the CPU's, in its order, with explicitly rounded fp32 operations (no FMA
 // contraction), so that every intermediate equals the scalar C code's; blocks are written in the file layout (18 / 144 bytes),
-// ready for b200_weight_upload or a GGCC file.  Creating a 40B-parameter synthetic model this way takes seconds
-// instead of the CPU quantiser's tens of minutes.
+// ready for b200_weight_upload or a GGCC file.
 #include "kernels.h"
 
 cudaStream_t b200_current_stream();
-bool launch_quantize_kquant(int ggml_type, const float * x_dev, void * blocks_dev, int64_t n_elems, cudaStream_t s);
+bool launch_quantize_kquant(int ggml_type, const float * x_dev, void * blocks_dev, int64_t nrows, int64_t row_blocks, cudaStream_t s);
 
 __device__ __forceinline__ int rne_int_dev(float v) {                 // nearest_int: the 1.5 * 2^23 magic constant
     const float t = __fadd_rn(v, 12582912.f);
@@ -65,18 +65,11 @@ __device__ __forceinline__ void pack_sm6_dev(int j, uint8_t * q, uint8_t ls, uin
     else { q[j + 4] = (uint8_t) ((ls & 0xF) | ((lm & 0xF) << 4)); q[j - 4] |= (uint8_t) ((ls >> 4) << 6); q[j] |= (uint8_t) ((lm >> 4) << 6); }
 }
 
-__global__ void __launch_bounds__(64) quantize_q4_K_kernel(const float * __restrict__ x, uint8_t * __restrict__ y, int64_t nblocks) {
-    const int64_t b = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= nblocks) return;
-    const float * xb = x + b * 256; uint8_t * yb = y + b * 144;
-    uint8_t L[256]; float mins[8], scales[8];
+// one Q4_K block.  L holds the codes of the row's previous block on entry (zeros for block 0) and this block's on exit.
+__device__ void quantize_q4_K_block(const float * __restrict__ xb, uint8_t * __restrict__ yb, uint8_t * L) {
+    float mins[8], scales[8];
     uint8_t sc[12];
     for (int i = 0; i < 12; i++) sc[i] = 0;
-    // make_qkx1_quants stops refining when a round leaves L unchanged, and in round 0 it compares against whatever the buffer held
-    // before: on the CPU that is the previous block's final codes (or uninitialised stack for the first block of a row,
-    // k_quants.c:548).  Here the buffer starts as zeros, so round 0 always counts as a change (some element gets level 15):
-    // identical to the CPU unless all 32 round-0 levels of a sub-block coincide with the stale bytes (probability ~16^-32 on
-    // non-degenerate data; constant sub-blocks take the mx == mn exit before any of this).
     float max_scale = 0.f, max_min = 0.f;
     for (int j = 0; j < 8; j++) {
         scales[j] = fit_scale_min_dev(xb + 32 * j, L + 32 * j, mins[j]);
@@ -103,17 +96,44 @@ __global__ void __launch_bounds__(64) quantize_q4_K_kernel(const float * __restr
     for (int j = 0; j < 256; j += 64) for (int l = 0; l < 32; l++) *q++ = (uint8_t) (L[j + l] | (L[j + l + 32] << 4));
 }
 
-// x_dev: n_elems fp32 values; blocks_dev: n_elems / block_elems blocks in the file layout.  Returns 0 if the type has no
-// device quantiser yet (callers quantise on the host then).
-extern "C" int b200_quantize_weights(int ggml_type, const float * x_dev, void * blocks_dev, int64_t n_elems) {
+// make_qkx1_quants stops refining after a round that leaves L unchanged, and its round 0 compares against whatever L held before:
+// quantize_row_q4_K_reference declares L once per call (k_quants.c:546), so block b of a row starts from block b-1's final codes.  Whenever a
+// sub-block's round-0 codes equal the ones 256 values earlier -- a repeated or rescaled sub-block does it -- the CPU stops after
+// round 0 where fresh codes would refine further.  So one thread walks a whole row and carries L; block 0 starts from zeros (the
+// CPU reads uninitialised stack there).
+__global__ void __launch_bounds__(32) quantize_q4_K_kernel(const float * __restrict__ x, uint8_t * __restrict__ y, int64_t nrows,
+                                                           int64_t row_blocks) {
+    const int64_t r = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= nrows) return;
+    uint8_t L[256];
+    for (int i = 0; i < 256; i++) L[i] = 0;
+    for (int64_t b = r * row_blocks; b < (r + 1) * row_blocks; b++) quantize_q4_K_block(x + b * 256, y + b * 144, L);
+}
+
+// x_dev: n_elems fp32 values, rows of row_len; blocks_dev: n_elems / block_elems blocks in the file layout.  Returns 1 on success
+// (n_elems == 0 launches nothing), 0 if the type has no device quantiser (callers quantise on the host then), -1 if row_len is not a
+// positive multiple of the type's block or n_elems not a non-negative multiple of row_len.
+extern "C" int b200_quantize_weights_rows(int ggml_type, const float * x_dev, void * blocks_dev, int64_t n_elems, int64_t row_len) {
+    const int64_t qk = ggml_type == T_Q4_0 ? 32 : 256;
+    if (ggml_type != T_Q4_0 && ggml_type != T_Q2_K && ggml_type != T_Q3_K && ggml_type != T_Q4_K && ggml_type != T_Q5_K &&
+        ggml_type != T_Q6_K) return 0;
+    if (row_len <= 0 || row_len % qk != 0 || n_elems < 0 || n_elems % row_len != 0) return -1;
+    if (n_elems == 0) return 1;
     cudaStream_t s = b200_current_stream();
-    if (ggml_type == T_Q4_0 && n_elems % 32 == 0) {
+    if (ggml_type == T_Q4_0) {
         const int64_t nb = n_elems / 32;
         quantize_q4_0_kernel<<<(unsigned) ((nb + 255) / 256), 256, 0, s>>>(x_dev, (uint8_t *) blocks_dev, nb);
-    } else if (ggml_type == T_Q4_K && n_elems % 256 == 0) {
-        const int64_t nb = n_elems / 256;
-        quantize_q4_K_kernel<<<(unsigned) ((nb + 63) / 64), 64, 0, s>>>(x_dev, (uint8_t *) blocks_dev, nb);
-    } else return launch_quantize_kquant(ggml_type, x_dev, blocks_dev, n_elems, s) ? 1 : 0;      // Q2_K / Q3_K / Q5_K / Q6_K: quant_gpu_k.cu
+    } else if (ggml_type == T_Q4_K) {
+        const int64_t nrows = n_elems / row_len;
+        quantize_q4_K_kernel<<<(unsigned) ((nrows + 31) / 32), 32, 0, s>>>(x_dev, (uint8_t *) blocks_dev, nrows, row_len / 256);
+    } else launch_quantize_kquant(ggml_type, x_dev, blocks_dev, n_elems / row_len, row_len / 256, s);      // quant_gpu_k.cu
     B200_CUDA_CHECK(cudaGetLastError());
     return 1;
+}
+
+// the whole buffer as ONE row: one call of quantize_row_q*_reference over n_elems values (what ggml_quantize_chunk does with a
+// chunk), so Q2_K / Q4_K / Q5_K carry their codes across the whole buffer on one thread -- for a matrix use the _rows entry point
+extern "C" int b200_quantize_weights(int ggml_type, const float * x_dev, void * blocks_dev, int64_t n_elems) {
+    return n_elems == 0 ? b200_quantize_weights_rows(ggml_type, x_dev, blocks_dev, 0, 256)
+                        : b200_quantize_weights_rows(ggml_type, x_dev, blocks_dev, n_elems, n_elems);
 }

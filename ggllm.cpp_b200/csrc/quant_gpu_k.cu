@@ -4,10 +4,11 @@
 //   Q3_K  quantize_row_q3_K_reference, k_quants.c:396-470     (make_q3_quants :163-220, 6-bit signed scales, high-bit mask)
 //   Q5_K  quantize_row_q5_K_reference, k_quants.c:652-732     (make_qkx1_quants on 8 sub-blocks of 32, 6-bit scales / mins, qh plane)
 //   Q6_K  quantize_row_q6_K_reference, k_quants.c:781-843     (make_qx_quants rmse_type 1 :57-161, int8 scales)
-// One thread per 256-value block, the block's arithmetic in the scalar C code's order.  THIS FILE IS COMPILED WITH --fmad=false
-// (csrc/Makefile): every a * b + c below is a separately rounded multiply and add, divisions are IEEE, so each intermediate equals
+// Q3_K / Q6_K: one thread per 256-value block.  Q2_K / Q5_K: one thread per row, walking its blocks in order and carrying
+// make_qkx1_quants's codes from block to block (quant_gpu.cu, quantize_q4_K_kernel, says why).  The arithmetic is the scalar C
+// code's, in its order.  THIS FILE IS COMPILED WITH --fmad=false (csrc/Makefile): every a * b + c below is a separately rounded multiply and add, divisions are IEEE, so each intermediate equals
 // the CPU's (the reference is built without fp contraction).  Blocks are written in the file layout (84 / 110 / 176 / 210 bytes).
-// With these a Falcon-40B / 180B model of any K-quant type is created in seconds instead of the CPU quantiser's tens of minutes.
+// A Falcon-40B ffn_up (32768 rows of 8192) takes 1-6 ms per type on an H100 80GB (tools/quantise_bench.py).
 #include "kernels.h"
 
 cudaStream_t b200_current_stream();
@@ -23,9 +24,8 @@ __device__ __forceinline__ void st16(uint8_t * p, uint16_t v) { *reinterpret_cas
 __device__ __forceinline__ int imin(int a, int b) { return a < b ? a : b; }
 __device__ __forceinline__ int imax(int a, int b) { return a > b ? a : b; }
 
-// make_qkx1_quants: asymmetric (scale, min) fit of n values to levels 0..nmax, up to 5 refinement rounds.  L must hold zeros on entry
-// (the CPU compares round 0 against whatever its buffer held before -- the previous block's codes; see quant_gpu.cu for why that
-// cannot matter on non-degenerate data).
+// make_qkx1_quants: asymmetric (scale, min) fit of n values to levels 0..nmax, up to 5 refinement rounds.  Round 0 compares against
+// what L holds on entry: the same sub-block's codes in the row's previous block, zeros in block 0.
 __device__ float fit_scale_min(int n, int nmax, const float * x, uint8_t * L, float & the_min) {
     float mn = x[0], mx = x[0];
     for (int i = 1; i < n; i++) { if (x[i] < mn) mn = x[i]; if (x[i] > mx) mx = x[i]; }
@@ -130,12 +130,9 @@ __device__ float fit_scale_sym(int n, int nmax, const float * x, int8_t * L) {
     return scale;
 }
 
-__global__ void __launch_bounds__(64) quantize_q2_K_kernel(const float * __restrict__ x, uint8_t * __restrict__ y, int64_t nblocks) {
-    const int64_t b = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= nblocks) return;
-    const float * xb = x + b * 256; uint8_t * yb = y + b * 84;
-    uint8_t L[256]; float mins[16], scales[16]; uint8_t sc[16];
-    for (int i = 0; i < 256; i++) L[i] = 0;
+// one block each; L carries the previous block's codes in and this block's out
+__device__ void quantize_q2_K_block(const float * __restrict__ xb, uint8_t * __restrict__ yb, uint8_t * L) {
+    float mins[16], scales[16]; uint8_t sc[16];
     float max_scale = 0.f, max_min = 0.f;
     for (int j = 0; j < 16; j++) {
         scales[j] = fit_scale_min(16, 3, xb + 16 * j, L + 16 * j, mins[j]);
@@ -216,12 +213,8 @@ __device__ __forceinline__ void pack_sm6(int j, uint8_t * q, uint8_t ls, uint8_t
     else { q[j + 4] = (uint8_t) ((ls & 0xF) | ((lm & 0xF) << 4)); q[j - 4] |= (uint8_t) ((ls >> 4) << 6); q[j] |= (uint8_t) ((lm >> 4) << 6); }
 }
 
-__global__ void __launch_bounds__(64) quantize_q5_K_kernel(const float * __restrict__ x, uint8_t * __restrict__ y, int64_t nblocks) {
-    const int64_t b = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= nblocks) return;
-    const float * xb = x + b * 256; uint8_t * yb = y + b * 176;
-    uint8_t L[256]; float mins[8], scales[8]; uint8_t sc[12], qh[32];
-    for (int i = 0; i < 256; i++) L[i] = 0;
+__device__ void quantize_q5_K_block(const float * __restrict__ xb, uint8_t * __restrict__ yb, uint8_t * L) {
+    float mins[8], scales[8]; uint8_t sc[12], qh[32];
     for (int i = 0; i < 12; i++) sc[i] = 0;
     float max_scale = 0.f, max_min = 0.f;
     for (int j = 0; j < 8; j++) {
@@ -258,6 +251,17 @@ __global__ void __launch_bounds__(64) quantize_q5_K_kernel(const float * __restr
     for (int i = 0; i < 32; i++) yb[16 + i] = qh[i];
 }
 
+// one thread per row: the blocks in order, L carried from each to the next and zero at the row's start
+template <void (*quantize_block)(const float *, uint8_t *, uint8_t *), int BLOCK_BYTES>
+__global__ void __launch_bounds__(32) quantize_rows_kernel(const float * __restrict__ x, uint8_t * __restrict__ y, int64_t nrows,
+                                                           int64_t row_blocks) {
+    const int64_t r = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= nrows) return;
+    uint8_t L[256];
+    for (int i = 0; i < 256; i++) L[i] = 0;
+    for (int64_t b = r * row_blocks; b < (r + 1) * row_blocks; b++) quantize_block(x + b * 256, y + b * BLOCK_BYTES, L);
+}
+
 __global__ void __launch_bounds__(64) quantize_q6_K_kernel(const float * __restrict__ x, uint8_t * __restrict__ y, int64_t nblocks) {
     const int64_t b = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= nblocks) return;
@@ -290,16 +294,16 @@ __global__ void __launch_bounds__(64) quantize_q6_K_kernel(const float * __restr
 
 } // namespace
 
-// returns false for a type this file does not cover
-bool launch_quantize_kquant(int ggml_type, const float * x_dev, void * blocks_dev, int64_t n_elems, cudaStream_t s) {
-    if (n_elems % 256 != 0) return false;
-    const int64_t nb = n_elems / 256;
-    const unsigned grid = (unsigned) ((nb + 63) / 64);
+// nrows rows of row_blocks 256-value blocks, nrows > 0; returns false for a type this file does not cover
+bool launch_quantize_kquant(int ggml_type, const float * x_dev, void * blocks_dev, int64_t nrows, int64_t row_blocks, cudaStream_t s) {
+    const int64_t nb = nrows * row_blocks;
+    const unsigned grid = (unsigned) ((nb + 63) / 64), row_grid = (unsigned) ((nrows + 31) / 32);
+    uint8_t * y = (uint8_t *) blocks_dev;
     switch (ggml_type) {
-        case T_Q2_K: quantize_q2_K_kernel<<<grid, 64, 0, s>>>(x_dev, (uint8_t *) blocks_dev, nb); break;
-        case T_Q3_K: quantize_q3_K_kernel<<<grid, 64, 0, s>>>(x_dev, (uint8_t *) blocks_dev, nb); break;
-        case T_Q5_K: quantize_q5_K_kernel<<<grid, 64, 0, s>>>(x_dev, (uint8_t *) blocks_dev, nb); break;
-        case T_Q6_K: quantize_q6_K_kernel<<<grid, 64, 0, s>>>(x_dev, (uint8_t *) blocks_dev, nb); break;
+        case T_Q2_K: quantize_rows_kernel<quantize_q2_K_block, 84><<<row_grid, 32, 0, s>>>(x_dev, y, nrows, row_blocks); break;
+        case T_Q3_K: quantize_q3_K_kernel<<<grid, 64, 0, s>>>(x_dev, y, nb); break;
+        case T_Q5_K: quantize_rows_kernel<quantize_q5_K_block, 176><<<row_grid, 32, 0, s>>>(x_dev, y, nrows, row_blocks); break;
+        case T_Q6_K: quantize_q6_K_kernel<<<grid, 64, 0, s>>>(x_dev, y, nb); break;
         default: return false;
     }
     B200_CUDA_CHECK(cudaGetLastError());

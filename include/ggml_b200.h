@@ -97,9 +97,15 @@ void   b200_mul_mat_vec_q(const b200_weight * w, const b200_actq * a, float * y_
  * libfalcon.cpp:2389-2394).  a_out must have K == rows of w and the activation type of the next weight.
  * returns 0 if the type / shape is not covered (rows % 256 != 0, or not Q4_K / Q4_0). */
 int    b200_mul_mat_vec_q_chain(const b200_weight * w, const b200_actq * a_in, float * y_dev, int epilogue, b200_actq * a_out);
-/* fp32 -> weight blocks in the FILE layout (18 B per 32 for Q4_0, 144 B per 256 for Q4_K) on the device, bit for bit what
- * quantize_row_q4_0_reference (ggml.c:927-962) / quantize_row_q4_K_reference (k_quants.c:542-605) write (SURVEY 8f-3).
- * Returns 0 for a type without a device quantiser (quantise on the host then), 1 on success. */
+/* b200_quantize_weights_rows: fp32 rows of row_len values -> weight blocks in the FILE layout on the device (Q4_0, Q2_K, Q3_K, Q4_K, Q5_K, Q6_K), every block
+ * of every row bit for bit what quantize_row_q*_reference (ggml.c:927-962, k_quants.c:275-843) writes when called once per row.
+ * Q2_K / Q4_K / Q5_K carry their fit's codes from block to block inside a row as the reference does; block 0 of a row starts from
+ * zeroed codes, where the reference reads uninitialised stack.  n_elems is a multiple of row_len.  Returns 1 on success
+ * (n_elems == 0 launches nothing), 0 for a type without a device quantiser (quantise on the host then), -1 for a bad shape
+ * (row_len not a positive multiple of the type's block, n_elems not a non-negative multiple of row_len). */
+int    b200_quantize_weights_rows(int ggml_type, const float * x_dev, void * blocks_dev, int64_t n_elems, int64_t row_len);
+/* the same with the whole buffer as one row: one call of quantize_row_q*_reference over n_elems values, as ggml_quantize_chunk makes
+ * for a chunk.  Q2_K / Q4_K / Q5_K then run the buffer on one thread: quantise matrices with b200_quantize_weights_rows. */
 int    b200_quantize_weights(int ggml_type, const float * x_dev, void * blocks_dev, int64_t n_elems);
 int    b200_mmv_max_n(void);
 /* which kernel the decode mat-vec (b200_mul_mat_vec_q / b200_mul_mat / b200_mul_mat_vec_q_chain) runs for a weight type and

@@ -384,9 +384,14 @@ static void unpack_q3_scales(const uint8_t *packed, int8_t out[16]) {
 
 /* =================================== Q2_K ====================================================== */
 /* block_q2_K {u8 scales[16]; u8 qs[64]; f16 d, dmin}: k_quants.h:20-26; quantize k_quants.c:275-342 */
-static void q2_K_enc(const float *x, uint8_t *y, int64_t k) {
-    uint8_t L[SB]; float mins[16], scales[16];
+/* make_qkx1_quants (Q2_K, Q4_K, Q5_K) ends its refinement after a round that leaves L unchanged, and its round 0 compares
+ * against what L already holds: the reference declares L once per call, so block b starts from block b-1's final codes.  That
+ * chaining is restated here.  For block 0 the reference reads uninitialised stack; here it reads zeros.  fresh != 0 zeroes L
+ * at every block instead, which is what a quantiser that treats blocks independently computes. */
+static void q2_K_enc(const float *x, uint8_t *y, int64_t k, int fresh) {
+    uint8_t L[SB] = {0}; float mins[16], scales[16];
     for (int64_t b = 0; b < k / SB; b++, x += SB, y += 84) {
+        if (fresh) memset(L, 0, sizeof L);
         uint8_t *sc = y, *qs = y + 16;
         float max_scale = 0, max_min = 0;
         for (int j = 0; j < 16; j++) {
@@ -489,10 +494,11 @@ static void q3_K_dec(const uint8_t *x, float *y, int64_t k) {
 /* =================================== Q4_K / Q5_K =============================================== */
 /* block_q4_K {f16 d, dmin; u8 scales[12]; u8 qs[128]}: k_quants.h:44-49; quantize k_quants.c:542-605
  * block_q5_K {f16 d, dmin; u8 scales[12]; u8 qh[32]; u8 qs[128]}: k_quants.h:56-63; quantize k_quants.c:652-732 */
-static void q45_K_enc(const float *x, uint8_t *y, int64_t k, int bits) {
+static void q45_K_enc(const float *x, uint8_t *y, int64_t k, int bits, int fresh) {   /* L chained as in q2_K_enc */
     const int nmax = (1 << bits) - 1; const size_t bsz = bits == 4 ? 144 : 176;
-    uint8_t L[SB]; float mins[8], scales[8];
+    uint8_t L[SB] = {0}; float mins[8], scales[8];
     for (int64_t b = 0; b < k / SB; b++, x += SB, y += bsz) {
+        if (fresh) memset(L, 0, sizeof L);
         uint8_t *sc = y + 4;
         float max_scale = 0, max_min = 0;
         for (int j = 0; j < 8; j++) {
@@ -643,14 +649,23 @@ int orc_quantize_row(int type, const float *x, void *y, int64_t k) {
         case ORC_Q5_1: q5_1_enc(x, o, k); return 0;
         case ORC_Q8_0: q8_0_enc_ref(x, o, k); return 0;
         case ORC_Q8_1: q8_1_enc_ref(x, o, k); return 0;
-        case ORC_Q2_K: q2_K_enc(x, o, k); return 0;
+        case ORC_Q2_K: q2_K_enc(x, o, k, 0); return 0;
         case ORC_Q3_K: q3_K_enc(x, o, k); return 0;
-        case ORC_Q4_K: q45_K_enc(x, o, k, 4); return 0;
-        case ORC_Q5_K: q45_K_enc(x, o, k, 5); return 0;
+        case ORC_Q4_K: q45_K_enc(x, o, k, 4, 0); return 0;
+        case ORC_Q5_K: q45_K_enc(x, o, k, 5, 0); return 0;
         case ORC_Q6_K: q6_K_enc(x, o, k); return 0;
         case ORC_Q8_K: q8_K_enc(x, o, k); return 0;
     }
     return -1;
+}
+int orc_quantize_row_fresh_codes(int type, const float *x, void *y, int64_t k) {
+    uint8_t *o = (uint8_t *)y;
+    switch (type) {
+        case ORC_Q2_K: q2_K_enc(x, o, k, 1); return 0;
+        case ORC_Q4_K: q45_K_enc(x, o, k, 4, 1); return 0;
+        case ORC_Q5_K: q45_K_enc(x, o, k, 5, 1); return 0;
+    }
+    return orc_quantize_row(type, x, y, k);
 }
 int orc_dequantize_row(int type, const void *x, float *y, int64_t k) {
     const uint8_t *i = (const uint8_t *)x;

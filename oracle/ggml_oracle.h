@@ -40,6 +40,11 @@ int    orc_vec_dot_type(int type);
  * quantize  : quantize_row_q*_reference (ggml.c:927-1129, 1292-1325; k_quants.c:275,396,542,652,781,899)
  * dequantize: dequantize_row_q*         (ggml.c:1509-1619; k_quants.c:344,472,607,734,845,936)          */
 int orc_quantize_row(int type, const float *x, void *y, int64_t k);
+/* orc_quantize_row with make_qkx1_quants's code buffer zeroed at every block (Q2_K, Q4_K, Q5_K; other types as
+ * orc_quantize_row).  orc_quantize_row carries the codes from block to block as the reference does (k_quants.c:275, 542,
+ * 652 declare L once per row); this variant computes every block on its own, so a case where the two differ is one where
+ * a quantiser that drops the carried codes would be wrong. */
+int orc_quantize_row_fresh_codes(int type, const float *x, void *y, int64_t k);
 int orc_dequantize_row(int type, const void *x, float *y, int64_t k);
 
 /* Q8_0 / Q8_1 activation quantisation as the x86 host executes it: the AVX/AVX2 bodies of

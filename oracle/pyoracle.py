@@ -60,6 +60,7 @@ class _Orc:
         L.orc_f16_to_f32.restype = C.c_float
         L.orc_f16_to_f32.argtypes = [C.c_uint16]
         L.orc_quantize_row.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int64]
+        L.orc_quantize_row_fresh_codes.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int64]
         L.orc_dequantize_row.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int64]
         L.orc_quantize_row_q8_0_x86.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
         L.orc_quantize_row_q8_1_x86.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
@@ -77,14 +78,16 @@ class _Orc:
         L.orc_falcon_eval_range.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int,
                                             C.c_int, C.c_int, C.c_void_p, C.c_void_p]
 
-    def quantize(self, t, x):
-        """x: float32 [..., k] -> uint8 [..., row_bytes] (quantize_row_q*_reference, row by row)."""
+    def quantize(self, t, x, fresh_codes=False):
+        """x: float32 [..., k] -> uint8 [..., row_bytes] (quantize_row_q*_reference, row by row).  fresh_codes: start every
+        block's make_qkx1_quants from zeroed codes instead of the previous block's (orc_quantize_row_fresh_codes)."""
         x = np.ascontiguousarray(x, dtype=np.float32)
         k = x.shape[-1]
         out = np.zeros(x.shape[:-1] + (row_bytes(t, k),), dtype=np.uint8)
         x2, o2 = x.reshape(-1, k), out.reshape(-1, out.shape[-1])
+        fn = self.L.orc_quantize_row_fresh_codes if fresh_codes else self.L.orc_quantize_row
         for r in range(x2.shape[0]):
-            assert self.L.orc_quantize_row(t, _fp(x2[r]), _fp(o2[r]), k) == 0
+            assert fn(t, _fp(x2[r]), _fp(o2[r]), k) == 0
         return out
 
     def quantize_act(self, wtype, x):
