@@ -17,12 +17,12 @@ PART_A = ["b200_event_create", "b200_event_destroy", "b200_event_record", "b200_
           "b200_stream_synchronize", "b200_init", "b200_device_count", "b200_set_stream", "b200_synchronize", "b200_malloc", "b200_free", "b200_memcpy_h2d",
           "b200_memcpy_d2h", "b200_memset", "b200_host_malloc", "b200_host_free", "b200_weight_upload", "b200_weight_random",
           "b200_weight_free", "b200_weight_device_bytes", "b200_dequantize_rows", "b200_actq_alloc", "b200_actq_free",
-          "b200_quantize_act", "b200_actq_download", "b200_actq_alloc_f16", "b200_actq_download_f16", "b200_actq_to_f16", "b200_mul_mat", "b200_mul_mat_f16", "b200_mul_mat_vec_q", "b200_mul_mat_vec_q_chain", "b200_quantize_weights", "b200_quantize_weights_rows", "b200_mmv_max_n", "b200_mmv_launch_shape", "b200_gemm_launch_shape", "b200_layernorm",
+          "b200_quantize_act", "b200_actq_download", "b200_actq_alloc_f16", "b200_actq_download_f16", "b200_actq_to_f16", "b200_mul_mat", "b200_mul_mat_f16", "b200_mul_mat_vec_q", "b200_mul_mat_vec_q_chain", "b200_quantize_weights", "b200_quantize_weights_rows", "b200_quantize_chunks", "b200_mmv_max_n", "b200_mmv_launch_shape", "b200_gemm_launch_shape", "b200_layernorm",
           "b200_gelu", "b200_add", "b200_rope_neox", "b200_attention", "b200_layernorm_q", "b200_attention_decode", "b200_attention_kv16", "b200_attention_decode_kv16",
           "b200_sampler_create", "b200_sampler_create_chain", "b200_sampler_sample", "b200_sampler_mirostat_mu", "b200_sampler_free",
           "b200_sampler_tap", "b200_sampler_tap_read", "b200_token_nll"]
 PART_B = ["b200_falcon_create", "b200_falcon_create_kv", "b200_falcon_kv_type", "b200_falcon_kv_device_bytes", "b200_falcon_set_tensor", "b200_falcon_set_tensor_random", "b200_falcon_load_ggcc",
-          "b200_ggcc_read_hparams", "b200_falcon_free", "b200_falcon_weight_bytes", "b200_nccl_unique_id",
+          "b200_ggcc_read_hparams", "b200_quantize_ggcc", "b200_falcon_free", "b200_falcon_weight_bytes", "b200_nccl_unique_id",
           "b200_falcon_init_pipeline", "b200_falcon_eval", "b200_falcon_decode_dev", "b200_falcon_logits_dev", "b200_falcon_generate_greedy",
           "b200_falcon_last_launches", "b200_attention_long_launches", "b200_falcon_last_ms", "b200_falcon_stream", "b200_falcon_profile_matvec",
           "b200_falcon_kv_read", "b200_falcon_kv_write", "b200_falcon_kv_shadow_read", "b200_falcon_kv_fill_random", "b200_falcon_generate", "b200_falcon_generate_chain", "b200_falcon_load_seconds", "b200_falcon_save_kv", "b200_falcon_load_kv",
@@ -58,7 +58,8 @@ def lib():
             "b200_actq_download": (None, [vp, vp, vp, vp, vp]),
             "b200_actq_alloc_f16": (vp, [i32, i64, i32]), "b200_actq_download_f16": (None, [vp, vp]), "b200_actq_to_f16": (None, [vp, vp, i64]),
             "b200_mul_mat": (None, [vp, vp, i64, i32, vp, i64]), "b200_mul_mat_vec_q": (None, [vp, vp, vp, i64, i32, vp, vp]),
-            "b200_mmv_max_n": (i32, []), "b200_mmv_launch_shape": (i32, [i32, i64, vp]), "b200_gemm_launch_shape": (i32, [i32, i64, i64, i32, i64, i32, vp]),"b200_mul_mat_vec_q_chain": (i32, [vp, vp, vp, i32, vp]), "b200_quantize_weights": (i32, [i32, vp, vp, i64]), "b200_quantize_weights_rows": (i32, [i32, vp, vp, i64, i64]), "b200_mul_mat_f16": (i32, [vp, vp, i64, i32, vp, i64, i32, i32]),
+            "b200_mmv_max_n": (i32, []), "b200_mmv_launch_shape": (i32, [i32, i64, vp]), "b200_gemm_launch_shape": (i32, [i32, i64, i64, i32, i64, i32, vp]),"b200_mul_mat_vec_q_chain": (i32, [vp, vp, vp, i32, vp]), "b200_quantize_weights": (i32, [i32, vp, vp, i64]), "b200_quantize_weights_rows": (i32, [i32, vp, vp, i64, i64]),
+            "b200_quantize_chunks": (i64, [i32, vp, vp, i64, i64, vp]), "b200_quantize_ggcc": (i32, [C.c_char_p, C.c_char_p, vp, vp]), "b200_mul_mat_f16": (i32, [vp, vp, i64, i32, vp, i64, i32, i32]),
             "b200_layernorm": (None, [vp, i64, vp, vp, vp, i64, i32, i32]), "b200_gelu": (None, [vp, vp, i64]), "b200_add": (None, [vp, vp, vp, i64]),
             "b200_rope_neox": (None, [vp, i32, i32, i32, i64, i32, i32, i32, f32, i32]),
             "b200_attention": (None, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32]),
@@ -336,6 +337,36 @@ class Sampler:
             self.free()
         except Exception:
             pass
+
+
+def quantize_chunks(ggml_type, x_dev, dst_dev, n_elems, chunk_elems, hist=None):
+    """b200_quantize_chunks: ggml_quantize_chunk over consecutive chunks of chunk_elems values (device pointers).  hist: an int64[16]
+    array the legacy code histograms are added to, or None.  -> bytes written, 0 for an unsupported type, -1 for a bad shape"""
+    hp = None
+    if hist is not None:
+        assert hist.dtype == np.int64 and hist.size == 16 and hist.flags.c_contiguous
+        hp = _np_ptr(hist)
+    return int(lib().b200_quantize_chunks(ggml_type, x_dev, dst_dev, n_elems, chunk_elems, hp))
+
+
+class QuantizeParams(C.Structure):
+    """b200_quantize_params: llama_model_quantize_params (nthread <= 0: the host's hardware threads)"""
+    _fields_ = [("nthread", C.c_int32), ("ftype", C.c_int32), ("allow_requantize", C.c_int32), ("quantize_output_tensor", C.c_int32)]
+
+
+class QuantizeReport(C.Structure):
+    _fields_ = [("size_org", C.c_uint64), ("size_new", C.c_uint64), ("hist", C.c_int64 * 16), ("n_tensors", C.c_int32),
+                ("n_quantized", C.c_int32), ("seconds", C.c_double), ("staging_bytes", C.c_uint64), ("device_bytes", C.c_uint64)]
+
+
+def quantize_ggcc(path_in, path_out, ftype, nthread=0, allow_requantize=False, quantize_output_tensor=True):
+    """b200_quantize_ggcc: falcon_quantize on the device -> (return code, QuantizeReport).  0: written; 1: the reference refuses
+    (unknown ftype, a k-quant of a row length not a multiple of 256, requantisation without allow_requantize); -1: unreadable or
+    malformed input, or an I/O error"""
+    p = QuantizeParams(nthread, ftype, int(bool(allow_requantize)), int(bool(quantize_output_tensor)))
+    r = QuantizeReport()
+    rc = lib().b200_quantize_ggcc(path_in.encode(), path_out.encode(), C.byref(p), C.byref(r))
+    return int(rc), r
 
 
 class FalconParams(C.Structure):

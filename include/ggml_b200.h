@@ -107,6 +107,15 @@ int    b200_quantize_weights_rows(int ggml_type, const float * x_dev, void * blo
 /* the same with the whole buffer as one row: one call of quantize_row_q*_reference over n_elems values, as ggml_quantize_chunk makes
  * for a chunk.  Q2_K / Q4_K / Q5_K then run the buffer on one thread: quantise matrices with b200_quantize_weights_rows. */
 int    b200_quantize_weights(int ggml_type, const float * x_dev, void * blocks_dev, int64_t n_elems);
+/* b200_quantize_chunks: ggml_quantize_chunk (ggml.c:19479-19560) on consecutive chunks of chunk_elems values of x_dev, the last chunk
+ * shorter, as falcon_quantize calls it (libfalcon.cpp:3662-3705); output in the file layout at dst_dev, bit for bit the reference's.
+ * Types: F16 (F16C rounding, NaN payloads kept), Q4_0, Q4_1, Q5_0, Q5_1, Q8_0, Q2_K, Q3_K, Q4_K, Q5_K, Q6_K.  Only Q2_K / Q4_K / Q5_K
+ * depend on the chunks: their fit carries codes from block to block within a chunk (zeroed at its start, where the reference reads
+ * uninitialised stack), one chain per chunk; chunk_elems == n_elems is one serial chain.  hist16 (host, 16 counts, or NULL) gets the
+ * reference's legacy code histograms added (the K-quants and F16 add nothing).  Synchronises when hist16 is given.  Returns the
+ * bytes written, 0 for a type outside the list, -1 for a bad shape (n_elems or chunk_elems not a multiple of the type's block,
+ * chunk_elems <= 0, n_elems < 0). */
+int64_t b200_quantize_chunks(int ggml_type, const float * x_dev, void * dst_dev, int64_t n_elems, int64_t chunk_elems, int64_t * hist16);
 int    b200_mmv_max_n(void);
 /* which kernel the decode mat-vec (b200_mul_mat_vec_q / b200_mul_mat / b200_mul_mat_vec_q_chain) runs for a weight type and
  * row length K.  Returns 1 and nt_j_d = {threads per CTA, pieces per thread, ring depth} for a tuned shape; 0 (nt_j_d = {0, 0, 0})
@@ -259,6 +268,36 @@ int           b200_falcon_load_ggcc(b200_falcon * f, const char * path);
 double        b200_falcon_load_seconds(const b200_falcon * f, size_t * bytes);
 /* hparams of a GGCC file without loading it (fills n_vocab..falcon_type); returns 0 on success */
 int           b200_ggcc_read_hparams(const char * path, b200_falcon_params * out);
+
+/* falcon_quantize on the device: mirrors llama_model_quantize_params (libfalcon.h) */
+typedef struct {
+    int32_t nthread;                 /* <= 0: the host's hardware threads.  Decides the chunk plan only: see b200_quantize_ggcc */
+    int32_t ftype;                   /* enum llama_ftype: 0 1 2 3 7 8 9 10 11 12 13 14 15 16 17 18 */
+    int32_t allow_requantize;        /* quantised input tensors may be dequantised and quantised again */
+    int32_t quantize_output_tensor;  /* 0: lm_head.weight is copied as it is (--leave-output-tensor) */
+} b200_quantize_params;
+typedef struct {
+    uint64_t size_org, size_new;     /* tensor data bytes in and out (falcon_quantize's "model size" / "quant size") */
+    int64_t  hist[16];               /* the legacy code histogram over every quantised tensor (zeros for F16 / K-quant outputs) */
+    int32_t  n_tensors, n_quantized;
+    double   seconds;                /* wall time, file open to file close */
+    uint64_t staging_bytes;          /* size of one pinned staging buffer: a tensor is read in pieces of at most this */
+    uint64_t device_bytes;           /* device memory the pipeline allocated */
+} b200_quantize_report;
+/* b200_quantize_ggcc: falcon_model_quantize (libfalcon.cpp:3533-3743) with the quantisers on the device: the output file is byte for
+ * byte the reference's.  A tensor is quantised iff its name ends in "weight", it is 2-D, it is not lm_head.weight when
+ * quantize_output_tensor is 0, and its type differs from the ftype's; every other tensor is copied.  F16 and quantised inputs are
+ * widened / dequantised on the device exactly as the reference converts them.  Chunk plan: nthread_use = nthread > 1 ?
+ * min(nthread, ceil(n / 16384)) : 1; with nthread_use < 2 a tensor is ONE chunk, otherwise chunks of 16384 values -- for Q2_K / Q4_K /
+ * Q5_K a single chunk is one serial chain over the whole tensor (slow for large tensors, and what the reference defines).
+ * Pipeline: the input is mapped; each tensor goes through pinned staging buffers (report->staging_bytes each) to the device, is
+ * converted, quantised and copied back while the host reads the next tensor and writes the previous one.  Device memory: two input
+ * buffers of the largest quantised tensor as stored, one fp32 buffer and one output buffer of it (about 10 bytes per value of the
+ * largest tensor for an F16 input).  The input is untrusted and bounds-checked as b200_falcon_load_ggcc checks it.  report may be
+ * NULL.  Returns 0 on success, 1 where the reference refuses (unknown ftype, a K-quant output for a tensor whose ne[0] is not a
+ * multiple of 256, a quantised input without allow_requantize; the output file is then not written), -1 for an unreadable or
+ * malformed input or an I/O error. */
+int           b200_quantize_ggcc(const char * path_in, const char * path_out, const b200_quantize_params * params, b200_quantize_report * report);
 void          b200_falcon_free(b200_falcon * f);
 size_t        b200_falcon_weight_bytes(const b200_falcon * f);   /* algorithmic bytes of the resident quantised matrices */
 
