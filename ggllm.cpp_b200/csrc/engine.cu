@@ -31,8 +31,6 @@
 #include <thread>
 #include <vector>
 
-cudaStream_t b200_current_stream();
-
 // ------------------------------------------------------------------------------------------------ NCCL (loaded lazily)
 struct NcclApi {
     void * lib = nullptr;

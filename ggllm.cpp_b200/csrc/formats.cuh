@@ -27,7 +27,7 @@ struct TypeSpec {
 };
 
 // plane 0 is always the main quant plane
-static inline TypeSpec type_spec(int t) {
+static constexpr TypeSpec type_spec(int t) {
     switch (t) {
         case T_F32:  return {1, 4, 1, {{0, 4}}};
         case T_F16:  return {1, 2, 1, {{0, 2}}};
@@ -85,6 +85,10 @@ static inline int act_type_for(int wtype) {
 __device__ __forceinline__ void unpack_sm6(int j, const uint8_t * s, int & sc, int & mn) {   // get_scale_min_k4, k_quants.c:264-271
     if (j < 4) { sc = s[j] & 63; mn = s[j + 4] & 63; }
     else { sc = (s[j + 4] & 0xF) | ((s[j - 4] >> 6) << 4); mn = (s[j + 4] >> 4) | ((s[j] >> 6) << 4); }
+}
+__device__ __forceinline__ void pack_sm6(int j, uint8_t * q, uint8_t ls, uint8_t lm) {     // its inverse (k_quants.c:565-578), for j = 0..7 in order
+    if (j < 4) { q[j] = ls; q[j + 4] = lm; }
+    else { q[j + 4] = (uint8_t) ((ls & 0xF) | ((lm & 0xF) << 4)); q[j - 4] |= (uint8_t) ((ls >> 4) << 6); q[j] |= (uint8_t) ((lm >> 4) << 6); }
 }
 __device__ __forceinline__ int q3_scale(const uint8_t * s, int j) {   // 6-bit scale j of the 12-byte q3_K field, bias kept (k_quants.c:486-493)
     const int lo = j < 8 ? (s[j] & 0xF) : (s[j - 8] >> 4);

@@ -36,7 +36,11 @@ struct MmvShape { int nt, j, d; };                  // NT threads per CTA, J pie
 MmvShape mmv_fast_pick_shape(int wtype, int K);     // the shape launch_mmv_fast launches
 bool   mmv_fast_supports(int wtype, int K);
 bool   mmv_fast_fills_sm(const WPlanes & W);       // its CTAs leave no registers for a side-stream kernel beside them
+// ---- c_api.cu
+cudaStream_t b200_current_stream();                 // the stream the C ABI's calls run on
+
 // ---- ops.cu
+unsigned ew_grid(int64_t n);                        // grid of the 256-thread grid-stride elementwise kernels: one thread per value, at most 132 * 16 CTAs
 void   launch_layernorm(const float * x, int64_t x_stride, const float * g, const float * b, float * y, int64_t y_stride,
                         int n, int rows, cudaStream_t stream);              // y = norm(x)*g + b ; g,b may be null (plain ggml_norm)
 // [x = (ra + rb) + x, written back] ; A1 = Q(norm(x)*g1+b1) ; A2 = Q(norm(x)*g2+b2) (optional) ; with y: rows r >= y_row0 also
@@ -165,6 +169,13 @@ bool   launch_gemm_tc(const WPlanes & W, const __half * X, int64_t x_stride, int
 // 16-byte aligned), nothing launched
 struct GemmTcShape { int bn, ksplit, producer; };
 GemmTcShape gemm_tc_pick_shape(int type, int64_t K, int64_t M, int N, int64_t x_stride, bool x_aligned, int epi_gelu);
+
+// ---- quant_gpu.cu: ggml_quantize_chunk (ggml.c:19479-19560) over consecutive chunks of `chunk` values, the last one shorter, for
+// every falcon_quantize output type but F32.  Only the carried types (make_qkx1_quants: Q2_K, Q4_K, Q5_K) see the chunks: one chain
+// per full chunk, and the short tail a second launch; every other type is one launch over the whole buffer.  hist_dev (16 counters,
+// or null) accumulates the legacy types' code histograms.  Returns the bytes written, 0 for any other type, -1 for a bad shape.
+int64_t launch_quantize_chunks(int ggml_type, const float * x, void * dst, int64_t n, int64_t chunk, unsigned long long * hist_dev,
+                               cudaStream_t s);
 
 // ---- sampling.cu: falcon_main's sampling chain on the device (logit bias, repetition / frequency / presence penalties, top-k,
 // tail-free, typical, top-p, temperature, mirostat 1 / 2, MT19937 draw)

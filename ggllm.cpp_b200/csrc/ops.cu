@@ -359,7 +359,7 @@ __global__ void scale_kernel(const float * __restrict__ a, float s, float * __re
 __global__ void f32_to_f16_kernel(const float * __restrict__ x, __half * __restrict__ y, int64_t n) {       // ggml_fp32_to_fp16_row
     for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x * blockDim.x) y[i] = __float2half_rn(x[i]);
 }
-static unsigned ew_grid(int64_t n) { int64_t g = (n + 255) / 256; return (unsigned) (g < 1 ? 1 : (g > 132 * 16 ? 132 * 16 : g)); }
+unsigned ew_grid(int64_t n) { int64_t g = (n + 255) / 256; return (unsigned) (g < 1 ? 1 : (g > 132 * 16 ? 132 * 16 : g)); }
 void launch_f32_to_f16(const float * x, __half * y, int64_t n, cudaStream_t s) { f32_to_f16_kernel<<<ew_grid(n), 256, 0, s>>>(x, y, n); B200_CUDA_CHECK(cudaGetLastError()); }
 void launch_gelu(const float * x, float * y, int64_t n, cudaStream_t s) { gelu_kernel<<<ew_grid(n), 256, 0, s>>>(x, y, n); B200_CUDA_CHECK(cudaGetLastError()); }
 void launch_add(const float * a, const float * b, float * y, int64_t n, cudaStream_t s) { add_kernel<<<ew_grid(n), 256, 0, s>>>(a, b, y, n); B200_CUDA_CHECK(cudaGetLastError()); }
