@@ -26,7 +26,7 @@ PART_B = ["b200_falcon_create", "b200_falcon_create_kv", "b200_falcon_kv_type", 
           "b200_falcon_init_pipeline", "b200_falcon_eval", "b200_falcon_decode_dev", "b200_falcon_logits_dev", "b200_falcon_generate_greedy",
           "b200_falcon_last_launches", "b200_attention_long_launches", "b200_falcon_last_ms", "b200_falcon_stream", "b200_falcon_profile_matvec",
           "b200_falcon_kv_read", "b200_falcon_kv_write", "b200_falcon_kv_shadow_read", "b200_falcon_kv_fill_random", "b200_falcon_generate", "b200_falcon_generate_chain", "b200_falcon_load_seconds", "b200_falcon_save_kv", "b200_falcon_load_kv",
-          "b200_falcon_tap", "b200_falcon_tap_read", "b200_falcon_score", "b200_falcon_perplexity", "b200_falcon_set_embeddings", "b200_falcon_embeddings"]
+          "b200_falcon_tap", "b200_falcon_tap_layers", "b200_falcon_tap_read", "b200_falcon_score", "b200_falcon_perplexity", "b200_falcon_set_embeddings", "b200_falcon_embeddings"]
 
 
 def build(verbose=False):
@@ -86,7 +86,7 @@ def lib():
             "b200_falcon_eval": (i32, [vp, vp, i32, i32, i32, vp, i32]), "b200_falcon_decode_dev": (i32, [vp, vp, i32, i32]), "b200_falcon_generate_greedy": (i32, [vp, i32, i32, i32, i32, vp]),
             "b200_falcon_logits_dev": (vp, [vp]), "b200_falcon_last_launches": (i32, [vp]), "b200_falcon_last_ms": (f32, [vp]),
             "b200_falcon_stream": (vp, [vp]), "b200_falcon_profile_matvec": (f32, [vp, i32, vp, vp]),
-            "b200_falcon_tap": (i32, [vp, i32]), "b200_falcon_tap_read": (i32, [vp, i32, C.c_char_p, vp, sz]),
+            "b200_falcon_tap": (i32, [vp, i32]), "b200_falcon_tap_layers": (i32, [vp, vp, i32]), "b200_falcon_tap_read": (i32, [vp, i32, C.c_char_p, vp, sz]),
             "b200_token_nll": (None, [vp, i32, i32, i64, vp, vp, vp]),
             "b200_falcon_score": (i32, [vp, vp, i32, i32, i32, vp, vp]), "b200_falcon_perplexity": (i32, [vp, vp, i32, i32, vp, vp]),
             "b200_falcon_set_embeddings": (i32, [vp, i32]), "b200_falcon_embeddings": (C.POINTER(C.c_float), [vp]),
@@ -524,6 +524,12 @@ class Falcon:
         """switch the test tap on (copies of every layer's intermediates, b200_falcon_tap) or off"""
         if self.L.b200_falcon_tap(self.h, int(bool(on))) != 0:
             raise RuntimeError("b200_falcon_tap failed")
+
+    def tap_layers(self, layers):
+        """switch the test tap on for the listed (global index) layers only (b200_falcon_tap_layers); the head is tapped too"""
+        ids = np.ascontiguousarray(layers, dtype=np.int32)
+        if self.L.b200_falcon_tap_layers(self.h, _np_ptr(ids), ids.size) != 0:
+            raise RuntimeError("b200_falcon_tap_layers: a layer that is not local or listed twice")
 
     def tap_read(self, layer, node, dtype, shape):
         """-> one tapped buffer of the most recent eval (layer -1: after the head) as an array of `dtype` and `shape`"""

@@ -111,11 +111,12 @@ struct b200_falcon {
     bool emb_on = false, emb_valid = false;
     float * emb_dev = nullptr, * emb_h = nullptr; const float * emb_src = nullptr;
     std::vector<const void *> borrowed;         // device planes adopted from another owner (ggml_cuda_transform_tensor): never freed here
-    // test tap (b200_falcon_tap): while mem is set, every eval copies its intermediates into mem -- one slice of layer_bytes per local
-    // layer at the end of that layer, then one slice after the head.  Node offsets are the same in every layer slice.
+    // test tap (b200_falcon_tap / _tap_layers): while mem is set, every eval copies its intermediates into mem -- one slice of layer_bytes
+    // per tapped local layer at the end of that layer, then one slice after the head.  Node offsets are the same in every layer slice.
     struct TapNode { std::string name; const void * src; size_t row_bytes, off; bool all_rows; };    // all_rows: N rows, else the head's rows
-    struct Tap { uint8_t * mem = nullptr; std::vector<TapNode> layer, head; size_t layer_bytes = 0; int rows = 0, head_rows = 0;
-                 std::vector<int> rotated; } tap;                // rotated[l]: RoPE ran in place on qkv (not inside the attention kernels)
+    struct Tap { uint8_t * mem = nullptr; std::vector<TapNode> layer, head; size_t layer_bytes = 0; int rows = 0, head_rows = 0, n_slices = 0;
+                 std::vector<int> rotated, slice; } tap;         // rotated[l]: RoPE ran in place on qkv (not inside the attention kernels);
+                                                                 // slice[l]: local layer l's slice, -1 when it is not tapped
 };
 
 // Local layer l's slice of the KV cache (kernels.h's KvCache): f32 rows of kv_row() floats, fp16 planes shadow_layer halves apart.
@@ -566,12 +567,12 @@ static void tap_copy(b200_falcon * f, const std::vector<b200_falcon::TapNode> & 
 static void tap_layer(b200_falcon * f, int l, int N) {
     if (!f->tap.mem) return;
     f->tap.rows = N;
-    tap_copy(f, f->tap.layer, f->tap.mem + (size_t) l * f->tap.layer_bytes);
+    if (f->tap.slice[l] >= 0) tap_copy(f, f->tap.layer, f->tap.mem + (size_t) f->tap.slice[l] * f->tap.layer_bytes);
 }
 static void tap_head(b200_falcon * f, int N, int nr) {
     if (!f->tap.mem) return;
     f->tap.rows = N; f->tap.head_rows = nr;
-    tap_copy(f, f->tap.head, f->tap.mem + (size_t) f->NL * f->tap.layer_bytes);
+    tap_copy(f, f->tap.head, f->tap.mem + (size_t) f->tap.n_slices * f->tap.layer_bytes);
 }
 
 // final LayerNorm + lm_head over rows x[0 .. nr) of the residual stream: libfalcon.cpp:2422-2440.  ra / rb (optional, quantised head
@@ -1207,12 +1208,13 @@ static void tap_add_actq(std::vector<b200_falcon::TapNode> & v, size_t & total, 
     tap_add(v, total, name + ".s", A.s, (size_t) (A.K / 32) * 4, NB, all_rows);
     tap_add(v, total, name + ".bs", A.bs, (size_t) (A.K / (A.type == T_Q8_K ? 16 : 32)) * 2, NB, all_rows);
 }
-int b200_falcon_tap(b200_falcon * f, int on) {
+// slice[l] >= 0 for the local layers that get a slice (tap on), or slice empty (tap off)
+static void tap_setup(b200_falcon * f, const std::vector<int> & slice) {
     invalidate_graphs(f);                                 // the captured decode graphs hold the copies (or their absence)
     B200_CUDA_CHECK(cudaDeviceSynchronize());
     B200_CUDA_CHECK(cudaFree(f->tap.mem));
     f->tap = b200_falcon::Tap{};
-    if (!on) return 0;
+    if (slice.empty()) return;
     ensure_actq(f);
     const int NB = f->hp.n_batch > 0 ? f->hp.n_batch : 1;
     const size_t E4 = (size_t) f->E * 4;
@@ -1235,16 +1237,34 @@ int b200_falcon_tap(b200_falcon * f, int on) {
         tap_add(T.head, hb, "logits", f->logits, (size_t) f->V * 4, NB, false);
     }
     T.layer_bytes = lb;
-    B200_CUDA_CHECK(cudaMalloc(&T.mem, lb * f->NL + hb + 256));
+    T.slice = slice;
+    for (int s : slice) T.n_slices += s >= 0;
+    B200_CUDA_CHECK(cudaMalloc(&T.mem, lb * T.n_slices + hb + 256));
     T.rotated.assign(f->NL, 0);
+}
+int b200_falcon_tap(b200_falcon * f, int on) {
+    std::vector<int> slice;
+    for (int l = 0; on && l < f->NL; l++) slice.push_back(l);
+    tap_setup(f, slice);
     return 0;
+}
+int b200_falcon_tap_layers(b200_falcon * f, const int * layers, int n) {
+    std::vector<int> slice(f->NL, -1);
+    bool ok = n > 0 && layers;
+    for (int i = 0; ok && i < n; i++) {
+        const int l = layers[i] - f->hp.layer_first;
+        ok = l >= 0 && l < f->NL && slice[l] < 0;
+        if (ok) slice[l] = i;
+    }
+    tap_setup(f, ok ? slice : std::vector<int>());
+    return ok ? 0 : 1;
 }
 int b200_falcon_tap_read(const b200_falcon * f, int layer, const char * node, void * host, size_t bytes) {
     const auto & T = f->tap;
     if (!T.mem || !node || !host) return 1;
     const bool head = layer == -1;
     const int l = layer - f->hp.layer_first;
-    if (head ? !f->last : (l < 0 || l >= f->NL)) return 1;
+    if (head ? !f->last : (l < 0 || l >= f->NL || T.slice[l] < 0)) return 1;
     if (!head && !strcmp(node, "qkv_rotated")) {
         if (bytes != sizeof(int)) return 1;
         memcpy(host, &T.rotated[l], sizeof(int));
@@ -1254,7 +1274,7 @@ int b200_falcon_tap_read(const b200_falcon * f, int layer, const char * node, vo
         if (n.name != node) continue;
         if (bytes != n.row_bytes * (n.all_rows ? T.rows : T.head_rows)) return 1;
         B200_CUDA_CHECK(cudaStreamSynchronize(f->s_main));
-        B200_CUDA_CHECK(cudaMemcpy(host, T.mem + (head ? (size_t) f->NL * T.layer_bytes : (size_t) l * T.layer_bytes) + n.off, bytes, cudaMemcpyDeviceToHost));
+        B200_CUDA_CHECK(cudaMemcpy(host, T.mem + (size_t) (head ? T.n_slices : T.slice[l]) * T.layer_bytes + n.off, bytes, cudaMemcpyDeviceToHost));
         return 0;
     }
     return 1;

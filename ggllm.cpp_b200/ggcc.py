@@ -121,8 +121,10 @@ def read_ggcc(path, mmap=True):
 
 
 def random_blocks(ggml_type, n_rows, k, rng):
-    """n_rows x k weights as well-formed pseudo-random blocks of `ggml_type` (uniform quant bytes, sane fp16 scales):
-    the host twin of b200_weight_random, for files the reference has to load (SURVEY.md section 8d)."""
+    """n_rows x k weights as well-formed pseudo-random blocks of `ggml_type` (uniform quant bytes, sane fp16 scales), drawn from
+    numpy's `rng`, for files the reference has to load (SURVEY.md section 8d).  Not the device's bytes: b200_weight_random hashes
+    its blocks with mix32, its F16 / F32 values lie in [0, 0.04) rather than 0.02 N(0, 1), and its Q4_1 / Q5_1 mins are 4 d;
+    tests/device_random.py is the byte-for-byte twin of those."""
     per, bsz = BLOCK[ggml_type]
     nb = n_rows * (k // per)
     if ggml_type == 0:

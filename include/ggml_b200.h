@@ -394,8 +394,12 @@ float         b200_falcon_profile_matvec(b200_falcon * f, int reps, int * n_laun
  *     "qkv_rotated" one int: 1 if RoPE rotated Q and K inside qkv, 0 if the attention kernels rotated them in registers.
  *   layer = -1 (last rank), after the head: "inp" the final residual [N][n_embd]; "xf.*" (quantised head) or "gen_na" (generic head) and
  *     "logits", each over the head's rows (the last one, or all N with all_logits).
- * Returns 0, or non-zero for a tap that is off, an unknown node, a layer that is not local or a wrong size. */
+ * Returns 0, or non-zero for a tap that is off, an unknown node, a layer that is not local or not tapped, or a wrong size.
+ * b200_falcon_tap_layers(f, layers, n) switches the tap on for the n listed (global index) layers only: a slice each plus the head's,
+ * so a prompt batch of a deep model can be checked a few layers at a time (one Falcon-40B slice at n_batch 512 is about 234 MB).
+ * Returns non-zero, with the tap off, for a layer that is not local or listed twice. */
 int           b200_falcon_tap(b200_falcon * f, int on);
+int           b200_falcon_tap_layers(b200_falcon * f, const int * layers, int n);
 int           b200_falcon_tap_read(const b200_falcon * f, int layer, const char * node, void * host, size_t bytes);
 /* number of kernel launches (graph nodes) issued by the most recent eval on this rank */
 int           b200_falcon_last_launches(const b200_falcon * f);

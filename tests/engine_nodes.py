@@ -72,10 +72,14 @@ class Model:
         t, ne, a = self.t[name]
         return np.ascontiguousarray(a).reshape(ne[1], -1)
 
+    def raw_rows(self, name, rows):
+        """the stored rows `rows` of a matrix (a model built lazily overrides this to make only those rows)"""
+        return self.raw(name)[rows]
+
     def rows(self, name, rows):
         """float32 dequantised rows of a matrix"""
         t, ne, _ = self.t[name]
-        r = self.raw(name)[rows]
+        r = self.raw_rows(name, rows)
         if t == po.F32:
             return r.view(np.float32) if r.dtype == np.uint8 else r.astype(np.float32)
         if t == po.F16:
@@ -204,9 +208,9 @@ def matmul_reference(m, wname, act, N, ev, rows):
         if N <= ev.mmv_max_n:
             y, b = np.zeros((N, len(rows))), np.zeros((N, len(rows)))
             s0 = s if s is not None else np.zeros((N, K // 32), np.float32)
-            wq = m.raw(wname)
+            wq = m.raw_rows(wname, rows)
             for n in range(N):
-                y[n], b[n], _, _ = mmv_exact.reference(t, wq, K, q[n], d[n], s0[n], ev.kernel_of(t, K), rows=rows)
+                y[n], b[n], _, _ = mmv_exact.reference(t, wq, K, q[n], d[n], s0[n], ev.kernel_of(t, K))
             return y, b
         x = actq_edges.f16_plane(po.VEC_DOT_TYPE[t], q, d).astype(np.float64)
     elif t == po.F16 and N > ev.mmv_max_n:
@@ -254,19 +258,35 @@ def check_matmul(node, layer, m, wname, got, act, ev, gelu=False, rope=None):
 
 
 # ------------------------------------------------------------------------------------------------ one eval
+def check_residuals(m, ev, residuals, head):
+    """(a) alone over every layer: residuals[l] = {"inp", "ao", "dn"} of layer l = 0 .. n_layer - 1 (a tap of those three nodes is
+    enough), head: the nodes after the head.  Raises NodeError at the first residual that is not exact."""
+    N, E = ev.N, m.E
+    want = m.rows("transformer.word_embeddings.weight", ev.tokens)
+    for l, nd in enumerate(list(residuals) + [head]):
+        got = nd["inp"].reshape(N, E)
+        need(np.array_equal(got.view(np.uint32), want.view(np.uint32)), "inp", l if l < len(residuals) else -1,
+             "not the embedding rows of the tokens" if l == 0 else "not (dn + ao) + inp of the layer before")
+        if l < len(residuals):
+            want = (nd["dn"].reshape(N, E) + nd["ao"].reshape(N, E)) + got
+
+
 def check_eval(m, ev, layers, head, rotated, layer_ids=None):
     """layers[i]: {node: array} of local layer layer_ids[i] (default 0, 1, ...), head: the nodes after the head (None on a rank without
-    it), rotated[i]: the tap's qkv_rotated.  Raises NodeError at the first node that fails."""
+    it), rotated[i]: the tap's qkv_rotated.  The residual check (a) links layer_ids[i] to layer_ids[i - 1] only where they are
+    consecutive, and the final residual to the last layer only where it is checked.  Raises NodeError at the first node that fails."""
     orc = po.orc()
     N, E, D, H, HKV = ev.N, m.E, m.D, m.H, m.HKV
     layer_ids = list(range(len(layers))) if layer_ids is None else layer_ids
     pos = ev.n_past + np.arange(N)
     T = ev.n_past + N
-    prev = None
+    prev, prev_l = None, None
     for i, (l, nd) in enumerate(zip(layer_ids, layers)):
         inp = nd["inp"].reshape(N, E)
         generic = "gen_nm" in nd
-        # (a)
+        # (a): linked to the layer before only where layer_ids holds it
+        if prev_l is not None and l != prev_l + 1:
+            prev = None
         if prev is None:
             if l == 0:
                 want = m.rows("transformer.word_embeddings.weight", ev.tokens)
@@ -274,6 +294,7 @@ def check_eval(m, ev, layers, head, rotated, layer_ids=None):
         else:
             want = (prev["dn"].reshape(N, E) + prev["ao"].reshape(N, E)) + prev["inp"].reshape(N, E)
             need(np.array_equal(inp.view(np.uint32), want.view(np.uint32)), "inp", l, "not (dn + ao) + inp of the layer before")
+        prev_l = l
         # (b)
         wq_name, wo_name, up_name, dn_name = (m.name(l, k) for k in ("qkv", "wo", "up", "down"))
         ln_m = orc.layernorm(inp, *m.ln(l, "mlp"))
@@ -362,11 +383,12 @@ def check_eval(m, ev, layers, head, rotated, layer_ids=None):
         prev = nd
     if head is None:
         return
-    # the head: (a) final residual, (b) LayerNorm, (c) lm_head, (g) returned logits
+    # the head: (a) final residual (when the last layer was checked), (b) LayerNorm, (c) lm_head, (g) returned logits
     nr = N - ev.r0
     fin = head["inp"].reshape(N, E)
-    want = (prev["dn"].reshape(N, E) + prev["ao"].reshape(N, E)) + prev["inp"].reshape(N, E)
-    need(np.array_equal(fin.view(np.uint32), want.view(np.uint32)), "inp", -1, "final residual is not (dn + ao) + inp of the last layer")
+    if prev is not None and prev_l == m.hp["n_layer"] - 1:
+        want = (prev["dn"].reshape(N, E) + prev["ao"].reshape(N, E)) + prev["inp"].reshape(N, E)
+        need(np.array_equal(fin.view(np.uint32), want.view(np.uint32)), "inp", -1, "final residual is not (dn + ao) + inp of the last layer")
     ln = orc.layernorm(fin[ev.r0:], m.t["transformer.ln_f.weight"][2], m.t["transformer.ln_f.bias"][2])
     lm = "lm_head.weight"
     t = m.wtype(lm)

@@ -26,8 +26,8 @@ def _kernel_of(t, K):
     return ("generic",) if s is None else ("fast", s[0], s[1])
 
 
-def read_tap(f, m, N, nr):
-    """{node: array} per local layer, the head's nodes and qkv_rotated per layer, of the most recent eval"""
+def read_tap(f, m, N, nr, layer_ids=None):
+    """{node: array} per local layer (or per layer of layer_ids), the head's nodes and qkv_rotated per layer, of the most recent eval"""
     E, FF = m.E, m.FF
     act = {}
     for name in ("transformer.h.0.self_attention.query_key_value.weight", "lm_head.weight"):
@@ -49,7 +49,7 @@ def read_tap(f, m, N, nr):
     for pre, K in (("xa", E), ("xm", E), ("xatt", E), ("xup", FF)):
         spec += actq_nodes(at, K, N, pre)
     layers, rotated = [], []
-    for l in range(m.hp["n_layer"]):
+    for l in range(m.hp["n_layer"]) if layer_ids is None else layer_ids:
         nd = {}
         for name, dt, shape in spec:
             try:

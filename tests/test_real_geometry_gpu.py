@@ -7,7 +7,8 @@ Falcon-7B 4544/71/1, Falcon-180B 14848/232/8), not only at the tiny test shapes:
   * the wgmma prompt attention over 16 key tiles (T = 2048) and the wgmma GEMM at the real K
   * whole evals (2 layers, vocabulary 2048) through b200_falcon_eval at those positions
 
-The 2-layer models carry well-formed pseudo-random blocks (ggcc.random_blocks: what bench.py's synthetic models hold) and the
+The 2-layer models carry well-formed pseudo-random blocks (ggcc.random_blocks: numpy-drawn blocks of the same kind as, but not the
+bytes of, the device-made weights bench.py times -- those are tests/device_random.py's, checked in test_bench_models_gpu.py) and the
 KV cache of BOTH the oracle and the engine is pre-filled with the same random rows (b200_falcon_kv_write), so a decode at
 position 8184 attends over a full context without 8184 evals first.
 
