@@ -21,7 +21,7 @@ PART_A = ["b200_event_create", "b200_event_destroy", "b200_event_record", "b200_
           "b200_gelu", "b200_add", "b200_rope_neox", "b200_attention", "b200_layernorm_q", "b200_attention_decode", "b200_attention_kv16", "b200_attention_decode_kv16",
           "b200_sampler_create", "b200_sampler_create_chain", "b200_sampler_sample", "b200_sampler_mirostat_mu", "b200_sampler_free",
           "b200_sampler_tap", "b200_sampler_tap_read", "b200_token_nll"]
-PART_B = ["b200_falcon_create", "b200_falcon_create_kv", "b200_falcon_kv_type", "b200_falcon_kv_device_bytes", "b200_falcon_set_tensor", "b200_falcon_set_tensor_random", "b200_falcon_load_ggcc",
+PART_B = ["b200_falcon_create", "b200_falcon_create_kv", "b200_falcon_create_streamed", "b200_falcon_stream_info", "b200_falcon_kv_type", "b200_falcon_kv_device_bytes", "b200_falcon_set_tensor", "b200_falcon_set_tensor_random", "b200_falcon_load_ggcc",
           "b200_ggcc_read_hparams", "b200_quantize_ggcc", "b200_falcon_free", "b200_falcon_weight_bytes", "b200_nccl_unique_id",
           "b200_falcon_init_pipeline", "b200_falcon_eval", "b200_falcon_decode_dev", "b200_falcon_logits_dev", "b200_falcon_generate_greedy",
           "b200_falcon_last_launches", "b200_attention_long_launches", "b200_falcon_last_ms", "b200_falcon_stream", "b200_falcon_profile_matvec",
@@ -78,6 +78,7 @@ def lib():
             "b200_falcon_load_seconds": (C.c_double, [vp, vp]),
             "b200_falcon_save_kv": (i32, [vp, C.c_char_p, i32]), "b200_falcon_load_kv": (i32, [vp, C.c_char_p]),
             "b200_falcon_create": (vp, [vp]), "b200_falcon_create_kv": (vp, [vp, i32]), "b200_falcon_kv_type": (i32, [vp]),
+            "b200_falcon_create_streamed": (vp, [vp, i32, vp, i32]), "b200_falcon_stream_info": (i32, [vp, vp, vp, vp, vp]),
             "b200_falcon_kv_device_bytes": (sz, [vp]), "b200_falcon_set_tensor": (None, [vp, C.c_char_p, i32, i32, vp, vp]),
             "b200_falcon_set_tensor_random": (None, [vp, C.c_char_p, i32, C.c_uint64]),
             "b200_falcon_load_ggcc": (i32, [vp, C.c_char_p]), "b200_ggcc_read_hparams": (i32, [C.c_char_p, vp]),
@@ -384,16 +385,24 @@ def layer_range(n_layer, rank, world):
 class Falcon:
     """The Falcon eval path (include/ggml_b200.h part B)."""
 
-    def __init__(self, hp, n_ctx, n_batch=1, rank=0, world=1, layers=None, kv_f16=False):
+    def __init__(self, hp, n_ctx, n_batch=1, rank=0, world=1, layers=None, kv_f16=False, streamed=()):
         """kv_f16: keep the KV cache in fp16 (b200_falcon_create_kv with GGML_TYPE_F16, the reference's f16_kv): half the cache bytes,
-        K / V rounded to fp16 as they are stored"""
+        K / V rounded to fp16 as they are stored.  streamed: global indices of layers whose matrices stay in pinned host memory and are
+        copied to the device for every eval (b200_falcon_create_streamed), for models larger than the card's memory"""
         self.L = lib()
         self.hp = dict(hp)
         lf, ll = layers if layers is not None else layer_range(hp["n_layer"], rank, world)      # layers: an explicit (first, last) range, e.g. balanced by bytes
         self.params = FalconParams(hp["n_vocab"], hp["n_embd"], hp["n_head"], hp["n_head_kv"], hp["n_layer"], hp["falcon_type"],
                                    n_ctx, n_batch, lf, ll, rank, world)
         self.layer_first, self.layer_last, self.rank, self.world = lf, ll, rank, world
-        self.h = self.L.b200_falcon_create_kv(C.byref(self.params), 1 if kv_f16 else 0)
+        streamed = np.ascontiguousarray(streamed, dtype=np.int32)
+        if streamed.size:
+            self.h = self.L.b200_falcon_create_streamed(C.byref(self.params), 1 if kv_f16 else 0, _np_ptr(streamed), streamed.size)
+            if not self.h:
+                raise ValueError("b200_falcon_create_streamed: streamed layers %s outside [%d, %d) or repeated, or world > 1"
+                                 % (streamed.tolist(), lf, ll))
+        else:
+            self.h = self.L.b200_falcon_create_kv(C.byref(self.params), 1 if kv_f16 else 0)
         self.n_vocab = hp["n_vocab"]
 
     @staticmethod
@@ -565,6 +574,14 @@ class Falcon:
 
     def stream(self):
         return self.L.b200_falcon_stream(self.h)
+
+    def stream_info(self):
+        """-> dict(layers, host_bytes, slot_bytes, copy_bytes) of the streamed layers (b200_falcon_stream_info)"""
+        n = self.L.b200_falcon_stream_info(self.h, None, None, None, None)
+        ids = np.zeros(max(n, 1), np.int32)
+        hb, sb, cb = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+        self.L.b200_falcon_stream_info(self.h, _np_ptr(ids), C.byref(hb), C.byref(sb), C.byref(cb))
+        return dict(layers=ids[:n].tolist(), host_bytes=hb.value, slot_bytes=sb.value, copy_bytes=cb.value)
 
     def weight_bytes(self):
         return self.L.b200_falcon_weight_bytes(self.h)

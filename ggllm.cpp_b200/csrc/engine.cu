@@ -23,6 +23,7 @@
 #include <sys/stat.h>
 #include <unistd.h>
 #include <algorithm>
+#include <array>
 #include <atomic>
 #include <chrono>
 #include <cmath>
@@ -117,6 +118,13 @@ struct b200_falcon {
     struct Tap { uint8_t * mem = nullptr; std::vector<TapNode> layer, head; size_t layer_bytes = 0; int rows = 0, head_rows = 0, n_slices = 0;
                  std::vector<int> rotated, slice; } tap;         // rotated[l]: RoPE ran in place on qkv (not inside the attention kernels);
                                                                  // slice[l]: local layer l's slice, -1 when it is not tapped
+    // Streamed layers (b200_falcon_create_streamed): their matrices live in pinned host images, in the device's planar bytes, and every
+    // eval copies each one into device slot rank % 2 on s_copy shortly before the layer runs.  A slot has one region per matrix role
+    // (wqkv, wo, up, down), sized to the largest streamed matrix of that role; a streamed WPlanes points into its slot for good, so
+    // the captured graphs bake in fixed addresses.  rank[l]: local layer l's position among the streamed layers, -1 when resident.
+    struct Streamed { std::vector<int> layers, rank; std::vector<std::array<uint8_t *, 4>> image;
+                      uint8_t * slot[2] = {}; size_t region[4] = {}, region_off[4] = {}, slot_bytes = 0;
+                      cudaStream_t s_copy = nullptr; cudaEvent_t e_fork = nullptr, e_join = nullptr, ready[2] = {}, free[2] = {}; } st;
 };
 
 // Local layer l's slice of the KV cache (kernels.h's KvCache): f32 rows of kv_row() floats, fp16 planes shadow_layer halves apart.
@@ -252,6 +260,87 @@ static void classify(b200_falcon * f) {
     f->classified = true;
 }
 
+// ---- streamed layers (b200_falcon::Streamed)
+static const WPlanes & role_matrix(const Layer & L, int r) { return r == 0 ? L.wqkv : r == 1 ? L.wo : r == 2 ? L.up : L.down; }
+static WPlanes & role_matrix(Layer & L, int r) { return const_cast<WPlanes &>(role_matrix((const Layer &) L, r)); }
+static int matrix_role(const Slot & s) {
+    switch (s.d->kind) { case S_QKV: return 0; case S_WO: return 1; case S_UP: return 2; case S_DOWN: return 3; default: return -1; }
+}
+static int stream_rank(const b200_falcon * f, int l) { return f->st.rank.empty() ? -1 : f->st.rank[l]; }
+static bool is_streamed(const b200_falcon * f, const Slot & s) {
+    return s.layer >= 0 && matrix_role(s) >= 0 && stream_rank(f, s.layer - f->hp.layer_first) >= 0;
+}
+static bool in_slot(const b200_falcon * f, const void * p) {
+    for (const uint8_t * s : f->st.slot) if (s && p >= s && p < s + f->st.slot_bytes) return true;
+    return false;
+}
+// Sizes the two slots for the streamed matrices laid out so far (reallocated only when a region changes size, which drops the graphs)
+// and points every one of them into its slot.
+static void stream_slots(b200_falcon * f) {
+    auto & S = f->st;
+    size_t need[4] = {};
+    for (int l : S.layers) for (int r = 0; r < 4; r++) need[r] = std::max(need[r], role_matrix(f->layers[l], r).bytes);
+    if (memcmp(need, S.region, sizeof(need)) != 0) {
+        invalidate_graphs(f);
+        B200_CUDA_CHECK(cudaDeviceSynchronize());
+        for (auto & p : S.slot) { B200_CUDA_CHECK(cudaFree(p)); p = nullptr; }
+        S.slot_bytes = 0;
+        for (int r = 0; r < 4; r++) { S.region[r] = need[r]; S.region_off[r] = S.slot_bytes; S.slot_bytes += need[r]; }
+        if (S.slot_bytes) for (auto & p : S.slot) B200_CUDA_CHECK(cudaMalloc(&p, S.slot_bytes));
+    }
+    for (size_t j = 0; j < S.layers.size(); j++)
+        for (int r = 0; r < 4; r++) {
+            WPlanes & W = role_matrix(f->layers[S.layers[j]], r);
+            if (W.bytes) wplanes_place(W, S.slot[j % 2] + S.region_off[r]);
+        }
+}
+// The planes of streamed matrix `s`, just built in its slot region, become its pinned host image.
+static void stream_store(b200_falcon * f, const Slot & s, const WPlanes & W, cudaStream_t st) {
+    uint8_t *& img = f->st.image[stream_rank(f, s.layer - f->hp.layer_first)][matrix_role(s)];
+    B200_ASSERT(!img);
+    B200_CUDA_CHECK(cudaHostAlloc(&img, W.bytes, cudaHostAllocDefault));
+    B200_CUDA_CHECK(cudaMemcpyAsync(img, W.p[0], W.bytes, cudaMemcpyDeviceToHost, st));
+    B200_CUDA_CHECK(cudaStreamSynchronize(st));
+}
+// The schedule on s_copy.  Streamed layer j's copy waits until layer j - 2 has released slot j % 2, then brings the four images over
+// and records ready[j % 2]; the first two copies go out when s_copy is forked from s_main at the start of the eval, beside the resident
+// layers in front of them.  A resident engine enqueues none of this.
+static void stream_copy(b200_falcon * f, int j) {
+    auto & S = f->st;
+    if (j >= 2) B200_CUDA_CHECK(cudaStreamWaitEvent(S.s_copy, S.free[j % 2], 0));
+    const Layer & L = f->layers[S.layers[j]];
+    for (int r = 0; r < 4; r++) {
+        const WPlanes & W = role_matrix(L, r);
+        if (S.image[j][r]) B200_CUDA_CHECK(cudaMemcpyAsync(W.p[0], S.image[j][r], W.bytes, cudaMemcpyHostToDevice, S.s_copy));
+    }
+    B200_CUDA_CHECK(cudaEventRecord(S.ready[j % 2], S.s_copy));
+}
+static void stream_fork(b200_falcon * f) {
+    auto & S = f->st;
+    if (S.layers.empty()) return;
+    B200_CUDA_CHECK(cudaEventRecord(S.e_fork, f->s_main));
+    B200_CUDA_CHECK(cudaStreamWaitEvent(S.s_copy, S.e_fork, 0));
+    for (int j = 0; j < (int) S.layers.size() && j < 2; j++) stream_copy(f, j);
+}
+static void stream_join(b200_falcon * f) {
+    auto & S = f->st;
+    if (S.layers.empty()) return;
+    B200_CUDA_CHECK(cudaEventRecord(S.e_join, S.s_copy));
+    B200_CUDA_CHECK(cudaStreamWaitEvent(f->s_main, S.e_join, 0));
+}
+// acquire: `st`, which is about to read local layer l's matrices, waits until they are in their slot.  release: every read of them has
+// been issued on s_main (the branches joined), so the slot may take the streamed layer after next.
+static void stream_acquire(b200_falcon * f, int l, cudaStream_t st) {
+    const int j = stream_rank(f, l);
+    if (j >= 0) B200_CUDA_CHECK(cudaStreamWaitEvent(st, f->st.ready[j % 2], 0));
+}
+static void stream_release(b200_falcon * f, int l) {
+    const int j = stream_rank(f, l);
+    if (j < 0) return;
+    B200_CUDA_CHECK(cudaEventRecord(f->st.free[j % 2], f->s_main));
+    if (j + 2 < (int) f->st.layers.size()) stream_copy(f, j + 2);
+}
+
 extern "C" {
 
 b200_falcon * b200_falcon_create(const b200_falcon_params * p) { return b200_falcon_create_kv(p, T_F32); }
@@ -302,6 +391,44 @@ b200_falcon * b200_falcon_create_kv(const b200_falcon_params * p, int kv_ggml_ty
     f->logits_h_floats = (size_t) f->V; B200_CUDA_CHECK(cudaMallocHost(&f->logits_h, f->logits_h_floats * 4));
     return f;
 }
+b200_falcon * b200_falcon_create_streamed(const b200_falcon_params * p, int kv_ggml_type, const int32_t * streamed_layers, int n_streamed) {
+    if (n_streamed == 0) return b200_falcon_create_kv(p, kv_ggml_type);
+    if (n_streamed < 0 || !streamed_layers || p->world > 1) return nullptr;
+    const int lf = p->layer_last <= 0 ? 0 : p->layer_first, ll = p->layer_last <= 0 ? p->n_layer : p->layer_last;
+    std::vector<int> layers;
+    for (int i = 0; i < n_streamed; i++) {
+        const int l = streamed_layers[i];
+        if (l < lf || l >= ll || std::find(layers.begin(), layers.end(), l - lf) != layers.end()) return nullptr;
+        layers.push_back(l - lf);
+    }
+    b200_falcon * f = b200_falcon_create_kv(p, kv_ggml_type);
+    if (!f) return nullptr;
+    auto & S = f->st;
+    std::sort(layers.begin(), layers.end());
+    S.layers = layers;
+    S.rank.assign(f->NL, -1);
+    for (size_t j = 0; j < layers.size(); j++) S.rank[layers[j]] = (int) j;
+    S.image.assign(layers.size(), {});
+    B200_CUDA_CHECK(cudaStreamCreateWithFlags(&S.s_copy, cudaStreamNonBlocking));
+    for (cudaEvent_t * e : { &S.e_fork, &S.e_join, &S.ready[0], &S.ready[1], &S.free[0], &S.free[1] })
+        B200_CUDA_CHECK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    return f;
+}
+int b200_falcon_stream_info(const b200_falcon * f, int32_t * layers_out, size_t * host_bytes, size_t * slot_bytes, size_t * copy_bytes) {
+    const auto & S = f->st;
+    size_t host = 0, copy = 0;
+    for (size_t j = 0; j < S.layers.size(); j++) {
+        if (layers_out) layers_out[j] = f->hp.layer_first + S.layers[j];
+        for (int r = 0; r < 4; r++) {
+            const size_t b = role_matrix(f->layers[S.layers[j]], r).bytes;
+            copy += b; if (S.image[j][r]) host += b;
+        }
+    }
+    if (host_bytes) *host_bytes = host;
+    if (slot_bytes) *slot_bytes = S.slot[0] ? 2 * S.slot_bytes : 0;
+    if (copy_bytes) *copy_bytes = copy;
+    return (int) S.layers.size();
+}
 
 static void ensure_actq(b200_falcon * f) {
     if (!f->attn_dec_scratch) {
@@ -334,6 +461,7 @@ static void ensure_actq(b200_falcon * f) {
 
 static void free_matrix(b200_falcon * f, WPlanes & W) {
     for (const void * b : f->borrowed) if (b == (const void *) W.p[0]) { W = WPlanes{}; return; }      // adopted: its owner frees it
+    if (in_slot(f, W.p[0])) { W = WPlanes{}; return; }                                                 // streamed: the slots are shared
     wplanes_free(W);
 }
 
@@ -344,6 +472,10 @@ static WPlanes & replace_matrix(b200_falcon * f, const Slot & s, int type) {
     WPlanes & W = *slot_dest(f, s).W;
     const bool counted = s.d->kind != S_EMB;
     if (W.p[0]) { if (counted) f->weight_bytes -= algorithmic_bytes(W.type, W.K, W.M); free_matrix(f, W); }
+    if (is_streamed(f, s)) {
+        uint8_t *& img = f->st.image[stream_rank(f, s.layer - f->hp.layer_first)][matrix_role(s)];
+        if (img) { B200_CUDA_CHECK(cudaFreeHost(img)); img = nullptr; }
+    }
     if (counted) f->weight_bytes += algorithmic_bytes(type, slot_K(f, s), slot_M(f, s));
     f->classified = false;
     return W;
@@ -351,10 +483,10 @@ static WPlanes & replace_matrix(b200_falcon * f, const Slot & s, int type) {
 
 // A weight matrix that is already resident in this library's planar layout (uploaded by ggml_cuda_transform_tensor for the reference's
 // loader, ggml_surface.cu) becomes the engine's matrix `name` without another copy.  Returns false for an unknown name / wrong shape /
-// a matrix of another rank.
+// a matrix of another rank or of a streamed layer.
 extern "C++" bool falcon_adopt_matrix(b200_falcon * f, const char * name, const WPlanes & W) {
     Slot s;
-    if (!find_slot(name, s) || !is_matrix(s) || !owns(f, s)) return false;
+    if (!find_slot(name, s) || !is_matrix(s) || !owns(f, s) || is_streamed(f, s)) return false;
     if (W.K != slot_K(f, s) || W.M != slot_M(f, s)) return false;
     replace_matrix(f, s, W.type) = W;
     f->borrowed.push_back((const void *) W.p[0]);
@@ -369,7 +501,12 @@ static void place_tensor(b200_falcon * f, const Slot & s, int type, const void *
     cudaStream_t st = f->s_main;
     if (is_matrix(s)) {
         WPlanes & W = replace_matrix(f, s, type);
-        if (random) wplanes_alloc_random(W, type, (int) K, (int) M, seed, st);
+        if (is_streamed(f, s)) {                    // built in its slot region, kept in its host image
+            wplanes_layout(W, type, (int) K, (int) M);
+            stream_slots(f);
+            if (random) wplanes_fill_random(W, seed, st); else wplanes_fill(W, host_data, st);
+            stream_store(f, s, W, st);
+        } else if (random) wplanes_alloc_random(W, type, (int) K, (int) M, seed, st);
         else wplanes_upload(W, type, (int) K, (int) M, host_data, st);
     } else {
         invalidate_graphs(f);
@@ -466,7 +603,9 @@ int b200_falcon_load_ggcc(b200_falcon * f, const char * path) {
     GgccHeader gh{}; gh.n_vocab = (uint32_t) hp.n_vocab;
     if (!ggcc_skip_vocab(c, gh)) return fail("truncated vocabulary");
     const double t0 = wall_seconds();
+    struct StreamItem { Slot s; const uint8_t * src; size_t row_bytes; };
     std::vector<LoadItem> items;
+    std::vector<StreamItem> streamed;
     size_t total = 0;
     for (;;) {
         GgccTensor t; const char * why = nullptr;
@@ -487,21 +626,43 @@ int b200_falcon_load_ggcc(b200_falcon * f, const char * path) {
             continue;
         }
         if (!owns(f, s)) continue;
-        WPlanes * W = &replace_matrix(f, s, (int) type);
-        wplanes_upload(*W, (int) type, (int) ne[0], (int) M, nullptr, f->s_main);  // planes allocated and laid out, filled below
         const int64_t chunk = (int64_t) (LOAD_BUF / row_bytes);
         if (chunk < 1) return fail("a row does not fit the staging buffer");
+        WPlanes * W = &replace_matrix(f, s, (int) type);
+        total += nbytes;
+        if (is_streamed(f, s)) {                                                   // laid out now, filled through a slot below
+            wplanes_layout(*W, (int) type, (int) ne[0], (int) M);
+            streamed.push_back({ s, data, row_bytes });
+            continue;
+        }
+        wplanes_upload(*W, (int) type, (int) ne[0], (int) M, nullptr, f->s_main);  // planes allocated and laid out, filled below
         for (int64_t r0 = 0; r0 < M; r0 += chunk) {
             const int64_t nr = r0 + chunk <= M ? chunk : M - r0;
             items.push_back({ W, data + (size_t) r0 * row_bytes, r0, nr, (size_t) nr * row_bytes });
         }
-        total += nbytes;
     }
     int dev; B200_CUDA_CHECK(cudaGetDevice(&dev));
     std::atomic<size_t> next(0);
     std::vector<std::thread> th;
     for (int t = 0; t < LOAD_THREADS; t++) th.emplace_back(load_worker, dev, &items, &next);
     for (auto & t : th) t.join();
+    // streamed matrices, one at a time through their slot region: raw rows H2D, the repack, the planes D2H into the host image
+    if (!streamed.empty()) {
+        stream_slots(f);
+        uint8_t * stage = nullptr;
+        B200_CUDA_CHECK(cudaMalloc(&stage, LOAD_BUF));
+        for (const StreamItem & it : streamed) {
+            const WPlanes & W = *slot_dest(f, it.s).W;
+            const int64_t chunk = (int64_t) (LOAD_BUF / it.row_bytes);
+            for (int64_t r0 = 0; r0 < W.M; r0 += chunk) {
+                const int64_t nr = std::min(chunk, (int64_t) W.M - r0);
+                B200_CUDA_CHECK(cudaMemcpyAsync(stage, it.src + (size_t) r0 * it.row_bytes, (size_t) nr * it.row_bytes, cudaMemcpyHostToDevice, f->s_main));
+                launch_repack_rows(W, stage, r0, nr, f->s_main);
+            }
+            stream_store(f, it.s, W, f->s_main);
+        }
+        B200_CUDA_CHECK(cudaFree(stage));
+    }
     munmap(map, (size_t) sb.st_size);
     f->load_seconds = wall_seconds() - t0; f->load_bytes = total;
     if (getenv("B200_VERBOSE")) fprintf(stderr, "b200: %s: %.2f GB of quantised matrices in %.2f s (%.1f GB/s)\n", path, total / 1e9, f->load_seconds, total / 1e9 / f->load_seconds);
@@ -524,6 +685,12 @@ void b200_falcon_free(b200_falcon * f) {
     for (auto & L : f->layers) { free_matrix(f, L.wqkv); free_matrix(f, L.wo); free_matrix(f, L.up); free_matrix(f, L.down);
         cudaFree(L.ln_attn_g); cudaFree(L.ln_attn_b); cudaFree(L.ln_mlp_g); cudaFree(L.ln_mlp_b); }
     free_matrix(f, f->tok_emb); free_matrix(f, f->lm_head);
+    for (auto & img : f->st.image) for (uint8_t * p : img) cudaFreeHost(p);
+    cudaFree(f->st.slot[0]); cudaFree(f->st.slot[1]);
+    if (f->st.s_copy) {
+        cudaStreamDestroy(f->st.s_copy);
+        for (cudaEvent_t e : { f->st.e_fork, f->st.e_join, f->st.ready[0], f->st.ready[1], f->st.free[0], f->st.free[1] }) cudaEventDestroy(e);
+    }
     cudaFree(f->lnf_g); cudaFree(f->lnf_b); cudaFree(f->kv.k); cudaFree(f->kv.v); cudaFree(f->kv.k16); cudaFree(f->kv.v16); cudaFree(f->kv.vt16);
     cudaFree(f->inp); cudaFree(f->qkv); cudaFree(f->att); cudaFree(f->ao); cudaFree(f->up); cudaFree(f->dn); cudaFree(f->logits);
     f->attn_scratch.release(); cudaFree(f->actq_mem); cudaFree(f->gen_na); cudaFree(f->gen_nm); cudaFree(f->gen_mm); cudaFree(f->xh_a); cudaFree(f->xh_b); cudaFree(f->xh_m);
@@ -612,8 +779,9 @@ static void ring_token_out(b200_falcon * f) {
 }
 
 // The residual stream's rows at the start of an eval: the embedding gather of the token ids on the first rank (libfalcon.cpp:2120),
-// the rows the previous rank sent on every other one
+// the rows the previous rank sent on every other one.  The streamed layers' copies start here.
 static void eval_input(b200_falcon * f, int N) {
+    stream_fork(f);
     if (f->first) {
         if (f->ring_mode && f->hp.world > 1) B200_NCCL_CHECK(nccl().Recv(f->tokens_dev, 1, ncclInt32, f->hp.world - 1, f->comm, f->s_main));
         launch_dequant_rows(f->tok_emb, f->tokens_dev, N, f->inp, f->E, f->s_main); f->launches++;
@@ -624,6 +792,7 @@ static void eval_input(b200_falcon * f, int N) {
 // the sampled id; on every other rank the rows go on to the next one.
 // fold_add: a quantised head's LayerNorm kernel does the adds (one kernel less on the decode step)
 static void eval_output(b200_falcon * f, int N, int logits_rows_from, bool fold_add) {
+    stream_join(f);
     const bool fold = fold_add && f->last && !f->generic_head && f->NL > 0;
     if (f->NL > 0 && !fold) { launch_add3(f->dn, f->ao, f->inp, f->inp, (int64_t) N * f->E, f->s_main); f->launches++; }
     if (!f->last) { B200_NCCL_CHECK(nccl().Send(f->inp, (size_t) N * f->E, ncclFloat, f->hp.rank + 1, f->comm, f->s_main)); return; }
@@ -686,6 +855,7 @@ static void enqueue_decode_fused(b200_falcon * f, int n_past, float theta_scale,
         if (dual) launch_layernorm_q(f->inp, E, ra, rb, E, L.ln_attn_g, L.ln_attn_b, &xa, L.ln_mlp_g, L.ln_mlp_b, &xm, E, 1, sa);
         else      launch_layernorm_q(f->inp, E, ra, rb, E, L.ln_mlp_g, L.ln_mlp_b, &xm, nullptr, nullptr, nullptr, E, 1, sa);
         f->launches++;
+        stream_acquire(f, l, sa);
         mmv(f, L.wqkv, dual ? xa : xm, f->qkv, f->QKV, none, sa);                                                // libfalcon.cpp:2192
         B200_CUDA_CHECK(cudaEventRecord(f->e_fork, sa));
         B200_CUDA_CHECK(cudaStreamWaitEvent(sb, f->e_fork, 0));
@@ -704,6 +874,7 @@ static void enqueue_decode_fused(b200_falcon * f, int n_past, float theta_scale,
         B200_CUDA_CHECK(cudaStreamWaitEvent(sa, f->e_join, 0));
         mmv(f, L.wo, xatt, f->ao, E, wo_epi, sa);                                                                // :2370
         if (wo_first) mmv(f, L.down, xup, f->dn, E, none, sa);
+        stream_release(f, l);
         tap_layer(f, l, 1);
     }
     eval_output(f, 1, 0, true);                                                      // :2399-2400, 2422-2440
@@ -721,11 +892,13 @@ static void enqueue_eval_generic(b200_falcon * f, int N, int n_past, float theta
         if (l > 0) { launch_add3(f->dn, f->ao, f->inp, f->inp, (int64_t) N * E, sa); f->launches++; }                 // :2399-2400
         launch_layernorm(f->inp, E, L.ln_mlp_g, L.ln_mlp_b, f->gen_nm, E, E, N, sa); f->launches++;                     // :2166-2185
         if (dual) { launch_layernorm(f->inp, E, L.ln_attn_g, L.ln_attn_b, f->gen_na, E, E, N, sa); f->launches++; }
+        stream_acquire(f, l, sa);
         mm_any(f, L.wqkv, dual ? f->gen_na : f->gen_nm, N, f->qkv, f->QKV, false, sa);                                   // :2192
         enqueue_attention(f, l, attn_params(f, l, N, n_past, theta_scale, graph_mode), sa);
         mm_any(f, L.wo, f->att, N, f->ao, E, false, sa);                                                                 // :2370
         mm_any(f, L.up, f->gen_nm, N, f->up, FF, true, sa);                                                              // :2389-2392
         mm_any(f, L.down, f->up, N, f->dn, E, false, sa);                                                                // :2394
+        stream_release(f, l);
         tap_layer(f, l, N);
     }
     eval_output(f, N, logits_rows_from, false);
@@ -754,11 +927,13 @@ static void enqueue_eval(b200_falcon * f, int N, int n_past, float theta_scale, 
         // fork: MLP branch on s_mlp
         B200_CUDA_CHECK(cudaEventRecord(f->e_fork, sa));
         B200_CUDA_CHECK(cudaStreamWaitEvent(sb, f->e_fork, 0));
+        stream_acquire(f, l, sb);
         f->launches += launch_mul_mat_q(L.up, xm, N, f->up, FF, EPI_GELU, sb);                                   // libfalcon.cpp:2389-2392
         launch_quantize_act(f->up, FF, xup, sb); f->launches++;
         f->launches += launch_mul_mat_q(L.down, xup, N, f->dn, E, EPI_NONE, sb);                                 // :2394
         B200_CUDA_CHECK(cudaEventRecord(f->e_join, sb));
         // attention branch on s_main
+        stream_acquire(f, l, sa);
         f->launches += launch_mul_mat_q(L.wqkv, dual ? xa : xm, N, f->qkv, f->QKV, EPI_NONE, sa);                // :2192
         AttnParams ap = attn_params(f, l, N, n_past, theta_scale, graph_mode);
         ap.fuse_rope = N == 1;                                                                                   // decode: RoPE + KV append inside the attention kernels
@@ -766,6 +941,7 @@ static void enqueue_eval(b200_falcon * f, int N, int n_past, float theta_scale, 
         launch_quantize_act(f->att, E, xatt, sa); f->launches++;
         f->launches += launch_mul_mat_q(L.wo, xatt, N, f->ao, E, EPI_NONE, sa);                                  // :2370
         B200_CUDA_CHECK(cudaStreamWaitEvent(sa, f->e_join, 0));                                                  // join
+        stream_release(f, l);
         tap_layer(f, l, N);
     }
     eval_output(f, N, logits_rows_from, false);
@@ -1289,8 +1465,8 @@ int b200_falcon_last_launches(const b200_falcon * f) { return f->launches; }
 float b200_falcon_last_ms(const b200_falcon * f) { return f->last_ms; }
 void * b200_falcon_stream(b200_falcon * f) { return (void *) f->s_main; }
 
-// Times the dominant kernel in isolation on the model's own matrices: every local quantised mat-vec (4 per layer +
-// lm_head) launched back to back on the eval stream, `reps` passes, CUDA events around the whole region.  Each
+// Times the dominant kernel in isolation on the model's own matrices: every local quantised mat-vec of the resident layers (4 per
+// layer; a streamed layer's matrices are in HBM only while an eval runs it) + lm_head launched back to back on the eval stream, `reps` passes, CUDA events around the whole region.  Each
 // launch reads a different matrix and one pass touches weight_bytes >> L2, so every launch streams cold HBM.
 // Returns the total milliseconds; *n_launches and *bytes describe the region (bytes = algorithmic weight bytes).
 float b200_falcon_profile_matvec(b200_falcon * f, int reps, int * n_launches, size_t * bytes) {
@@ -1305,7 +1481,9 @@ float b200_falcon_profile_matvec(b200_falcon * f, int reps, int * n_launches, si
     MmvEpilogue e = { EPI_NONE, nullptr, nullptr };
     int n = 0; size_t b = 0;
     auto pass = [&](bool count) {
-        for (auto & L : f->layers) {
+        for (int l = 0; l < f->NL; l++) {
+            if (stream_rank(f, l) >= 0) continue;
+            const Layer & L = f->layers[l];
             launch_mmv(L.wqkv, xe, f->qkv, f->QKV, e, st); launch_mmv(L.wo, xe, f->ao, f->E, e, st);
             launch_mmv(L.up, xe, f->up, f->FF, e, st); launch_mmv(L.down, xff, f->dn, f->E, e, st);
             if (count) { n += 4; b += algorithmic_bytes(L.wqkv.type, L.wqkv.K, L.wqkv.M) + algorithmic_bytes(L.wo.type, L.wo.K, L.wo.M)

@@ -6,6 +6,10 @@
 size_t wplanes_layout(WPlanes & W, int type, int K, int M);
 void   wplanes_upload(WPlanes & W, int type, int K, int M, const void * host_raw, cudaStream_t stream);
 void   wplanes_alloc_random(WPlanes & W, int type, int K, int M, uint64_t seed, cudaStream_t stream);
+// the two halves of the above, for planes that live in memory the caller provides: place a laid-out matrix at `base`, then fill it
+void   wplanes_place(WPlanes & W, uint8_t * base);
+void   wplanes_fill(const WPlanes & W, const void * host_raw, cudaStream_t stream);
+void   wplanes_fill_random(const WPlanes & W, uint64_t seed, cudaStream_t stream);
 void   launch_repack_rows(const WPlanes & W, const void * stage_dev, int64_t row0, int64_t nrows, cudaStream_t stream);   // raw blocks of rows [row0, row0 + nrows) -> planes
 void   wplanes_free(WPlanes & W);
 void   launch_dequant_rows(const WPlanes & W, const int32_t * rows_dev, int nrows, float * dst, int64_t dst_stride, cudaStream_t stream);

@@ -42,34 +42,47 @@ __global__ void repack_kernel(const uint8_t * __restrict__ src, WPlanes W, TypeS
     }
 }
 
-// Upload `M` rows of raw ggml blocks (host pointer, row-major, rows of K/blk blocks) to the device in planar
-// form.  Staged through a bounded pinned-size device scratch so a 100 GB model never needs 2x its size.
-void wplanes_upload(WPlanes & W, int type, int K, int M, const void * host_raw, cudaStream_t stream) {
-    const TypeSpec ts = type_spec(type);
+// Points the planes of a laid-out (or already placed) matrix at `base`, one allocation of W.bytes, keeping their offsets.
+void wplanes_place(WPlanes & W, uint8_t * base) {
+    const int n = type_spec(W.type).n_planes;
+    const uint8_t * p0 = W.p[0];
+    for (int i = n - 1; i >= 0; i--) W.p[i] = base + (size_t) (W.p[i] - p0);
+}
+
+static void wplanes_alloc(WPlanes & W, int type, int K, int M) {
     wplanes_layout(W, type, K, M);
     uint8_t * base = nullptr;
     B200_CUDA_CHECK(cudaMalloc(&base, W.bytes));
-    for (int i = 0; i < ts.n_planes; i++) W.p[i] = base + reinterpret_cast<size_t>(W.p[i]);
-    if (!host_raw) return;
+    wplanes_place(W, base);
+}
+
+// Fill a placed matrix from `M` rows of raw ggml blocks (host pointer, row-major, rows of K/blk blocks), in planar form.  Staged
+// through a bounded device scratch so a 100 GB model never needs 2x its size.
+void wplanes_fill(const WPlanes & W, const void * host_raw, cudaStream_t stream) {
+    const TypeSpec ts = type_spec(W.type);
+    const size_t M = (size_t) W.M;
     const size_t row_bytes = (size_t) W.nb * ts.blk_bytes;
-    const size_t chunk_rows = ts.n_planes == 1 ? (size_t) M : (size_t) ((256u << 20) / row_bytes > 0 ? (256u << 20) / row_bytes : 1);
     if (ts.n_planes == 1) {   // f32 / f16: rows are already planar; strided copy handles the 16 B row padding
         B200_CUDA_CHECK(cudaMemcpy2DAsync(W.p[0], W.stride[0], host_raw, row_bytes, row_bytes, M, cudaMemcpyHostToDevice, stream));
         B200_CUDA_CHECK(cudaStreamSynchronize(stream));
         return;
     }
+    const size_t chunk_rows = (256u << 20) / row_bytes > 0 ? (256u << 20) / row_bytes : 1;
     uint8_t * stage = nullptr;
-    const size_t stage_rows = chunk_rows < (size_t) M ? chunk_rows : (size_t) M;
+    const size_t stage_rows = chunk_rows < M ? chunk_rows : M;
     B200_CUDA_CHECK(cudaMalloc(&stage, stage_rows * row_bytes));
-    for (size_t r0 = 0; r0 < (size_t) M; r0 += stage_rows) {
-        const size_t nr = r0 + stage_rows <= (size_t) M ? stage_rows : (size_t) M - r0;
+    for (size_t r0 = 0; r0 < M; r0 += stage_rows) {
+        const size_t nr = r0 + stage_rows <= M ? stage_rows : M - r0;
         B200_CUDA_CHECK(cudaMemcpyAsync(stage, (const uint8_t *) host_raw + r0 * row_bytes, nr * row_bytes, cudaMemcpyHostToDevice, stream));
-        const int64_t n = (int64_t) nr * W.nb;
-        repack_kernel<<<(unsigned) ((n + 255) / 256), 256, 0, stream>>>(stage, W, ts, (int64_t) r0, (int64_t) nr);
-        B200_CUDA_CHECK(cudaGetLastError());
+        launch_repack_rows(W, stage, (int64_t) r0, (int64_t) nr, stream);
     }
     B200_CUDA_CHECK(cudaStreamSynchronize(stream));
     B200_CUDA_CHECK(cudaFree(stage));
+}
+
+void wplanes_upload(WPlanes & W, int type, int K, int M, const void * host_raw, cudaStream_t stream) {
+    wplanes_alloc(W, type, K, M);
+    if (host_raw) wplanes_fill(W, host_raw, stream);
 }
 
 // rows [row0, row0 + nrows) of an allocated matrix from their raw blocks staged on the device (the streaming loader, engine.cu)
@@ -131,14 +144,13 @@ __global__ void fill_random_kernel(WPlanes W, TypeSpec ts, uint64_t seed) {
         }
     }
 }
-void wplanes_alloc_random(WPlanes & W, int type, int K, int M, uint64_t seed, cudaStream_t stream) {
-    const TypeSpec ts = type_spec(type);
-    wplanes_layout(W, type, K, M);
-    uint8_t * base = nullptr;
-    B200_CUDA_CHECK(cudaMalloc(&base, W.bytes));
-    for (int i = 0; i < ts.n_planes; i++) W.p[i] = base + reinterpret_cast<size_t>(W.p[i]);
-    fill_random_kernel<<<132 * 8, 256, 0, stream>>>(W, ts, seed);
+void wplanes_fill_random(const WPlanes & W, uint64_t seed, cudaStream_t stream) {
+    fill_random_kernel<<<132 * 8, 256, 0, stream>>>(W, type_spec(W.type), seed);
     B200_CUDA_CHECK(cudaGetLastError());
+}
+void wplanes_alloc_random(WPlanes & W, int type, int K, int M, uint64_t seed, cudaStream_t stream) {
+    wplanes_alloc(W, type, K, M);
+    wplanes_fill_random(W, seed, stream);
 }
 
 // dst[r][e] = dequant(W[rows[r]][e]) -- ggml_get_rows on a quantised matrix (ggml.c:11975-12002), also the

@@ -253,6 +253,14 @@ b200_falcon * b200_falcon_create(const b200_falcon_params * params);
  * even (ggml_fp32_to_fp16 on an F16C host; beyond +-65504 a value becomes +-Inf) and every attention read widens them exactly: the
  * engine computes what the f32 engine would over a cache whose rows were rounded when they were appended.  It takes half the bytes. */
 b200_falcon * b200_falcon_create_kv(const b200_falcon_params * params, int kv_ggml_type);
+/* b200_falcon_create_kv whose layers streamed_layers[0..n_streamed) (global indices inside [layer_first, layer_last), no repeats) keep their
+ * four matrices in pinned host memory in the device's planar layout.  Each eval copies every streamed layer into one of two device
+ * layer slots just before the layer runs, overlapped with the layers before it.  Results are bit for bit those of the resident engine.
+ * n_streamed == 0 is b200_falcon_create_kv.  NULL for a bad layer list, a bad kv type, or world > 1. */
+b200_falcon * b200_falcon_create_streamed(const b200_falcon_params * params, int kv_ggml_type, const int32_t * streamed_layers, int n_streamed);
+/* number of streamed layers; layers_out (optional) gets them in ascending order.  host_bytes: the pinned images; slot_bytes: the two
+ * device slots; copy_bytes: what one eval copies host -> device (the sum of the streamed layers' images).  Any pointer may be NULL. */
+int           b200_falcon_stream_info(const b200_falcon * f, int32_t * layers_out, size_t * host_bytes, size_t * slot_bytes, size_t * copy_bytes);
 int           b200_falcon_kv_type(const b200_falcon * f);            /* GGML_TYPE_F32 or GGML_TYPE_F16 */
 size_t        b200_falcon_kv_device_bytes(const b200_falcon * f);   /* the cache plus any fp16 copy, all local layers */
 void          b200_falcon_set_tensor(b200_falcon * f, const char * name, int ggml_type, int n_dims,
@@ -299,7 +307,7 @@ typedef struct {
  * malformed input or an I/O error. */
 int           b200_quantize_ggcc(const char * path_in, const char * path_out, const b200_quantize_params * params, b200_quantize_report * report);
 void          b200_falcon_free(b200_falcon * f);
-size_t        b200_falcon_weight_bytes(const b200_falcon * f);   /* algorithmic bytes of the resident quantised matrices */
+size_t        b200_falcon_weight_bytes(const b200_falcon * f);   /* algorithmic bytes of the quantised matrices, streamed layers' included */
 
 /* NCCL pipeline plumbing (world > 1): rank 0 creates the id, every rank passes the same 128 bytes. */
 void          b200_nccl_unique_id(void * id128);
@@ -374,7 +382,8 @@ int           b200_falcon_generate_chain(b200_falcon * f, const b200_sampling_ch
                                          int32_t first_token, int n_past, int n_steps, int n_ctx_rope, int32_t * tokens_out);
 /* the cudaStream_t the eval path runs on (for event timing) */
 void *        b200_falcon_stream(b200_falcon * f);
-/* roofline probe: every resident quantised mat-vec of this rank (4 per layer + lm_head) launched back to back,
+/* roofline probe: every quantised mat-vec of this rank's resident layers (4 per layer; streamed layers are left out, their matrices
+ * are in HBM only while an eval runs them) + lm_head launched back to back,
  * `reps` passes, timed with CUDA events on the eval stream.  Returns total ms; fills the launch count and the
  * algorithmic weight bytes streamed in that region. */
 float         b200_falcon_profile_matvec(b200_falcon * f, int reps, int * n_launches, size_t * bytes);
@@ -401,7 +410,7 @@ float         b200_falcon_profile_matvec(b200_falcon * f, int reps, int * n_laun
 int           b200_falcon_tap(b200_falcon * f, int on);
 int           b200_falcon_tap_layers(b200_falcon * f, const int * layers, int n);
 int           b200_falcon_tap_read(const b200_falcon * f, int layer, const char * node, void * host, size_t bytes);
-/* number of kernel launches (graph nodes) issued by the most recent eval on this rank */
+/* number of kernel launches (graph nodes) issued by the most recent eval on this rank; a streamed layer's copies are not counted */
 int           b200_falcon_last_launches(const b200_falcon * f);
 int           b200_attention_long_launches(void);     /* diagnostics: launches (eager or captured) of the long-context decode attention kernels so far */
 /* CUDA-event time (ms) of the most recent eval's device work on this rank */
